@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""bench.py -- aggregated edges/s of the PNA layer forward on B200 (BASELINE.json metric), one JSON line.
+"""bench.py -- aggregated edges/s of the PNA layer forward on H100 (BASELINE.json metric), one JSON line.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one pass of the hot path over the whole graph: CSR (resident, built once) -> [N, 12*F] aggregation
-(mean/max/min/std x identity/amplification/attenuation) -- the kernels of libpna_sm100.so and nothing else.
+(mean/max/min/std x identity/amplification/attenuation) -- the kernels of libpna_sm90.so and nothing else.
   value        edges/s of that step, inputs resident in HBM, CUDA events around each step, L2 flushed between steps
   e2e          edges/s of PNAConvSimple.forward(x, edge_index) called with pinned HOST tensors: H2D of x and
                edge_index, CSR build, aggregation, post-MLP, D2H of the layer output, all inside the timed region
@@ -19,6 +19,9 @@ N = 1: BASELINE.json configs[1] (ogbn-arxiv-shaped, 169 343 nodes / 1 166 243 ed
 N > 1: bench_multi.py -- configs[3] at N = 4 (graph-batch shard), configs[4] at N = 8 (destination partition + halo exchange),
        configs[4] at N/8 scale otherwise.
 --impl reference: the same workload's reference op sequence on the host cores (rank 0 only), same config / steps / warm-up.
+--dump-outputs DIR (N = 1): after the timed steps, DIR/aggregate.npy holds a fixed, seeded sample of DUMP_ROWS rows of the
+last timed step's [N, 12*F] output (float32) and DIR/aggregate_rows.npy their row indices (float64): inputs are seeded, so two
+builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -37,6 +40,19 @@ if ROOT not in sys.path:
 
 import bench_common as bc                                   # noqa: E402
 from bench_common import AGGRS, SCALERS, METRIC, UNIT        # noqa: E402
+
+DUMP_ROWS = 8192      # 8192 rows x 1536 fp32 = 50 MB: under the 64 MB a dump may take
+
+
+def dump_sample(out: torch.Tensor, directory: str) -> None:
+    """Seeded row sample of `out` -> DIR/aggregate.npy (float32) + DIR/aggregate_rows.npy (float64 row indices)."""
+    import numpy as np
+    g = torch.Generator().manual_seed(0)
+    rows = torch.sort(torch.randperm(out.size(0), generator=g)[:DUMP_ROWS]).values
+    sample = out[rows.to(out.device)].float().cpu()
+    os.makedirs(directory, exist_ok=True)
+    np.save(os.path.join(directory, "aggregate.npy"), sample.numpy())
+    np.save(os.path.join(directory, "aggregate_rows.npy"), rows.double().numpy())
 
 
 def config2_dict(n, e, f, max_deg):
@@ -325,7 +341,7 @@ def run_ours(args):
         pna_b200.aggregate_forward(xd, csr, AGGRS, SCALERS, avg_deg, out=out, **kw)
 
     # clocks / throttle reasons are sampled (20 Hz) while the GPU runs this workload: the timed steps themselves last
-    # only ~15 ms, so the sampler brackets them with extra untimed passes of the same kernels to collect enough samples
+    # only tens of ms, so the sampler brackets them with extra untimed passes of the same kernels to collect enough samples
     with bc.ClockSampler(local) as clk:
         time.sleep(0.06)
         t_end = time.perf_counter() + 0.5
@@ -333,6 +349,8 @@ def run_ours(args):
             step()
         torch.cuda.synchronize()
         per_step = bc.timed_steps(step, args.steps, args.warmup, flush)
+        if args.dump_outputs:
+            dump_sample(out, args.dump_outputs)
         t_end = time.perf_counter() + 0.5
         while time.perf_counter() < t_end:
             step()
@@ -351,13 +369,6 @@ def run_ours(args):
     bytes_ = synth.algorithmic_bytes(n, e, f, 4, 12 * f)
     peak, peak_src = bc.measured_peaks()
     achieved = bytes_["b_min"] / (t_ms * 1e-3) / 1e9
-    traffic = None
-    prof = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(prof):
-        try:
-            traffic = json.load(open(prof)).get("dram_bytes_per_step")
-        except Exception:
-            traffic = None
 
     # e2e: the public layer call with HOST buffers (pinned), copies inside the timed region
     torch.manual_seed(0)
@@ -436,7 +447,7 @@ def run_ours(args):
         "ms_per_step": t_ms, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32",
         "data": "synthetic", "config": config2_dict(n, e, f, csr.max_degree),
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": traffic, "peak_source": peak_src, "bytes_model": "B_min = N*F*s + 4E + 4(N+1) + 12*N*F*s",
+                     "traffic": None, "peak_source": peak_src, "bytes_model": "B_min = N*F*s + 4E + 4(N+1) + 12*N*F*s",
                      "b_min_bytes": bytes_["b_min"], "b_gather_bytes": bytes_["b_gather"],
                      "effective_gbs_b_gather": bytes_["b_gather"] / (t_ms * 1e-3) / 1e9},
         "parity": {"ok": par["ok"], "parity_max_err": max(par["max_err_light"], par["max_err_split_vs_f64"]),
@@ -446,12 +457,11 @@ def run_ours(args):
                    "what": "every row of the timed step's output vs the CPU oracle (fp32 op sequence; rows split across warps vs float64)"},
         "kernels_ms": {"step_min": min(per_step), "step_median": statistics.median(per_step), "split_rows": csr.n_hubs,
                        "kernels": ("k_rows_stream (rows + chunks of split rows, split rows finalized by the last-arriving warp)"
-                                   if fold_finalize_enabled() else "k_rows_stream (rows + chunks of split rows) + k_hub_finalize")
-                                  + "; per-kernel times: profiles/"},
+                                   if fold_finalize_enabled() else "k_rows_stream (rows + chunks of split rows) + k_hub_finalize")},
         "layer_fwd": {"ms": full_ms, "edges_per_s": e / (full_ms * 1e-3), "ms_via_12f_tensor": full_ms_12f,
                       "what": "PNAConvSimple.forward, CSR cached: aggregation with the identity scaler ([N,4F]) + post-MLP linear on "
                               "the tensor cores regenerating the scaled copies in registers (pna_linear_scaled_fwd, 3xTF32 "
-                              "tcgen05); ms_via_12f_tensor = same layer through the materialised [N,12F] tensor"},
+                              "wgmma); ms_via_12f_tensor = same layer through the materialised [N,12F] tensor"},
         "csr_build_ms": {"first_call": csr_ms_first, "steady": csr_ms, "steady_wall": csr_wall_ms},
         "e2e": {"value": e / (e2e_ms * 1e-3), "unit": UNIT, "ms_per_step": e2e_ms,
                 "h2d_bytes_per_step": x.numel() * 4 + ei.numel() * 8, "d2h_bytes_per_step": n * f * 4,
@@ -475,8 +485,13 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true", help="skip the CPU leg (profiling runs)")
     ap.add_argument("--no-side-configs", action="store_true", help="skip the `configs` sub-object (profiling runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write a seeded sample of the last timed step's output to DIR/*.npy (N = 1)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
+    if args.dump_outputs and (args.impl != "ours" or args.gpus != 1 or int(os.environ.get("WORLD_SIZE", "1")) != 1
+                              or os.environ.get("PNA_BENCH_FORCE_MULTI") == "1"):
+        ap.error("--dump-outputs is implemented for the single-GPU CUDA path only (--impl ours --gpus 1)")
     if args.impl == "reference":
         return run_reference(args)
     return run_ours(args)

@@ -1,8 +1,8 @@
-/* The C ABI of libpna_sm100.so used from plain C (what a cgo / JNI / N-API binding would wrap): build the CSR of a tiny
+/* The C ABI of libpna_sm90.so used from plain C (what a cgo / JNI / N-API binding would wrap): build the CSR of a tiny
  * graph, run the PNA aggregation (mean max min std x identity amplification attenuation), print two rows.
  *
  *   gcc -std=c99 -I include -I /usr/local/cuda/include examples/c_caller.c -o /tmp/c_caller \
- *       -L pna_b200 -l:libpna_sm100.so -L /usr/local/cuda/lib64 -lcudart -Wl,-rpath,$PWD/pna_b200 && /tmp/c_caller
+ *       -L pna_b200 -l:libpna_sm90.so -L /usr/local/cuda/lib64 -lcudart -Wl,-rpath,$PWD/pna_b200 && /tmp/c_caller
  *
  * Reference being replaced: PNAConvSimple.aggregate, models/pytorch_geometric/pna.py:242-249. */
 #include <math.h>

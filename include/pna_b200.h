@@ -1,5 +1,5 @@
 /*
- * pna_b200.h -- C ABI of libpna_sm100.so, the B200 (sm_100a) PNA aggregation path.
+ * pna_b200.h -- C ABI of libpna_sm90.so, the H100 (sm_90a) PNA aggregation path.
  *
  * This is the drop-in boundary for ONE hot path of lukecavabarrett/pna: the
  * neighbourhood aggregation of the PNA layer (gather of source features, the
@@ -74,7 +74,7 @@ enum pna_flags {
 
 enum pna_query_what {
   PNA_QUERY_ABI_VERSION = 0,
-  PNA_QUERY_SM_ARCH = 1,          /* 100 : compiled for sm_100a only */
+  PNA_QUERY_SM_ARCH = 1,          /*  90 : compiled for sm_90a only */
   PNA_QUERY_DEFAULT_SPLIT = 2,    /* default in-degree at which a row is split across warps */
   PNA_QUERY_DEFAULT_CHUNK = 3,    /* default edges per chunk of a split row */
   PNA_QUERY_DEVICE_SM_COUNT = 4,  /* multiProcessorCount of the current device (needs a GPU) */
@@ -147,7 +147,7 @@ int pna_csr_light_view(const int32_t* rowptr, const int32_t* col, int64_t n_node
                        void* workspace, size_t workspace_bytes, pna_stream_t stream);
 int pna_csr_light_view_workspace_bytes(int64_t n_nodes, size_t* bytes);
 
-/* ---- the aggregation ("single hand-written sm_100a CUDA kernel", north_star) ------------------------------
+/* ---- the aggregation ("single hand-written sm_90a CUDA kernel", north_star) ------------------------------
  * For every destination row i (PyG semantics; In(i) = slots rowptr[i]..rowptr[i+1], d = |In(i)|):
  *   m_s   = gathered[col[s]] (+ row_bias[i] when given)          s in In(i)           pna.py:137-150 / :239-240
  *   sum   = fp32 sum of m_s in slot order;  mean = sum / max(d,1)                      aggregators.py:9-14
@@ -287,7 +287,7 @@ int pna_peer_barrier(const void* const* peer_flags, int32_t rank, int32_t world,
 /* ---- first dense linear of the post-aggregation MLP on the tensor cores (north_star: "the post-MLP uses tensor
  * cores only for its dense linear"; reference pna.py:222-227 post_nn[0], models/dgl/pna_layer.py:31 posttrans) -----
  * y[n_rows, n_out] = a[n_rows, n_in] . weight[n_out, n_in]^T + bias, fp32 in / fp32 out, fp32-accurate: every operand
- * is split hi + lo and three tcgen05.mma kind::tf32 products (hi.hi + hi.lo + lo.hi) accumulate in TMEM, because plain
+ * is split hi + lo and three wgmma tf32 products (hi.hi + hi.lo + lo.hi) accumulate in registers, because plain
  * TF32 (10-bit mantissa) cannot meet the 1e-5 parity bar.  n_in % 32 == 0, n_out in {64, 128, 256}; other shapes
  * return PNA_ERR_UNSUPPORTED and the caller keeps its library GEMM.  workspace: 2 * n_in * n_out floats (split weight). */
 int pna_linear_workspace_bytes(int32_t n_in, int32_t n_out, size_t* bytes);

@@ -242,10 +242,27 @@ def round2_cases():
                                   posttrans_layers=1, divide_input=True), state_dict=layd.state_dict(), out=outd))
 
 
+def live_case():
+    """The reference's PNAConvSimple.propagate on fresh random inputs (tests/test_oracle.py::test_live_reference_over_shims)."""
+    torch.manual_seed(5)
+    n, e, f = 300, 2000, 24
+    x = torch.randn(n, f)
+    ei = torch.randint(0, n, (2, e))
+    deg = deg_hist(ei[1], n)
+    aggrs = ["mean", "min", "max", "std"]
+    conv = PNAConvSimple(f, f, aggrs, S3, deg)
+    agg = conv.propagate(ei, x=x, size=None)
+    save("pyg_simple_live", dict(kind="pyg_simple_propagate", x=x, edge_index=ei, aggregators=aggrs, scalers=S3,
+                                 avg_deg=conv.avg_deg, aggregate=agg))
+
+
 if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     if "--round2" in sys.argv:
         round2_cases()
+        sys.exit(0)
+    if "--live" in sys.argv:
+        live_case()
         sys.exit(0)
     simple_case("pyg_simple_f16", 200, 900, 16, seed=1)
     simple_case("pyg_simple_f64_hub", 100, 400, 64, seed=2, hub=700)

@@ -1,4 +1,4 @@
-"""pna_b200 -- the PNA message-passing layer forward of lukecavabarrett/pna, rebuilt for B200 (sm_100a).
+"""pna_b200 -- the PNA message-passing layer forward of lukecavabarrett/pna, rebuilt for H100 (sm_90a).
 
 One hot path only (SURVEY.md section 8): destination-sorted CSR + one hand-written aggregation kernel
 (gather, mean/max/min/std, degree scalers, concatenated output) behind the reference's own layer signatures.

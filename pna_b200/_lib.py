@@ -1,4 +1,4 @@
-"""ctypes binding of ``libpna_sm100.so`` (the C ABI declared in ``include/pna_b200.h``).
+"""ctypes binding of ``libpna_sm90.so`` (the C ABI declared in ``include/pna_b200.h``).
 
 The shared library is the product; this module only loads it, mirrors its structs and turns its status
 codes into exceptions.  There is deliberately NO fallback: if the library is missing or a call fails the caller
@@ -13,7 +13,7 @@ import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 REPO_ROOT = os.path.dirname(_HERE)
-LIB_PATH = os.environ.get("PNA_B200_LIB") or os.path.join(_HERE, "libpna_sm100.so")   # env override: tuning builds only
+LIB_PATH = os.environ.get("PNA_B200_LIB") or os.path.join(_HERE, "libpna_sm90.so")   # env override: tuning builds only
 CUDA_SOURCES = [os.path.join(_HERE, "csrc", n) for n in
                 ("pna_aggregate.cu", "pna_aggregate_f32_vec.cu", "pna_aggregate_f32_scalar.cu", "pna_aggregate_bf16_vec.cu",
                  "pna_aggregate_bf16_scalar.cu", "pna_aggregate_f32_fsplit.cu", "pna_aggregate_bwd.cu", "pna_linear.cu", "pna_csr.cu", "pna_peer.cu", "pna_misc.cu")]
@@ -21,10 +21,10 @@ CUDA_HEADERS = [os.path.join(_HERE, "csrc", n) for n in ("common.cuh", "pna_aggr
     os.path.join(REPO_ROOT, "include", "pna_b200.h")]
 BUILD_DIR = os.path.join(_HERE, "csrc", "build")
 
-# sm_100a only: -gencode arch=compute_100a,code=sm_100a (no PTX for other targets, no multi-arch fat binary)
+# sm_90a only: -gencode arch=compute_90a,code=sm_90a (no PTX for other targets, no multi-arch fat binary)
 # -fmad=false: the accumulation must round the product m*m before adding it (reference: src * src, then scatter_add);
 # ptxas contracts mul.rn.f32x2 + add.rn.f32x2 into FFMA2 otherwise.  IEEE div/sqrt keep their explicit FMAs.
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-fmad=false", "-Xcompiler", "-fPIC"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-fmad=false", "-Xcompiler", "-fPIC"]
 
 # status codes / enums of include/pna_b200.h
 ABI_VERSION = 8
@@ -43,10 +43,10 @@ EXPORTED_SYMBOLS = ("pna_csr_workspace_bytes", "pna_csr_build", "pna_csr_light_v
 
 
 class PnaError(RuntimeError):
-    """A libpna_sm100 call returned a negative status; the message is pna_last_error()."""
+    """A libpna_sm90 call returned a negative status; the message is pna_last_error()."""
 
     def __init__(self, status: int, message: str):
-        super().__init__(f"libpna_sm100 status {status}: {message}")
+        super().__init__(f"libpna_sm90 status {status}: {message}")
         self.status = status
 
 
@@ -89,7 +89,7 @@ class AggStruct(C.Structure):
 
 
 def build_library(force: bool = False, verbose: bool = False, extra_flags=()) -> str:
-    """Compile libpna_sm100.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+    """Compile libpna_sm90.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     Every .cu is compiled to an object file in parallel (they are independent translation units), then linked with
     ``nvcc -shared``.  Objects are rebuilt when their source or any header is newer.
@@ -118,7 +118,7 @@ def build_library(force: bool = False, verbose: bool = False, extra_flags=()) ->
     with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as ex:
         logs = list(ex.map(run, jobs))
     if jobs or not os.path.exists(LIB_PATH) or os.path.getmtime(LIB_PATH) < max(os.path.getmtime(o) for o in objs):
-        run(["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB_PATH] + objs)
+        run(["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", LIB_PATH] + objs)
     if verbose and extra_flags:
         print("\n".join(logs))
     return LIB_PATH
@@ -139,7 +139,7 @@ def lib() -> C.CDLL:
         if not os.path.exists(LIB_PATH):
             raise ImportError(
                 f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a).  pna_b200 has no CPU or PyTorch fallback for its kernels.")
+                "(nvcc, sm_90a).  pna_b200 has no CPU or PyTorch fallback for its kernels.")
         L = C.CDLL(LIB_PATH)
         L.pna_last_error.restype = C.c_char_p
         L.pna_last_error.argtypes = []
@@ -187,7 +187,7 @@ def lib() -> C.CDLL:
         if abi != ABI_VERSION:
             raise ImportError(f"{LIB_PATH} has ABI version {abi}, this package needs {ABI_VERSION}: rebuild it")
         if L.pna_query(QUERY_SIZEOF_CSR) != C.sizeof(CsrStruct) or L.pna_query(QUERY_SIZEOF_AGG) != C.sizeof(AggStruct):
-            raise ImportError("ctypes struct layout does not match include/pna_b200.h: rebuild libpna_sm100.so")
+            raise ImportError("ctypes struct layout does not match include/pna_b200.h: rebuild libpna_sm90.so")
         _lib = L
     return _lib
 

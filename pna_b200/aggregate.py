@@ -1,4 +1,4 @@
-"""``pna_aggregate``: the PNA neighbourhood aggregation as one call into libpna_sm100.so.
+"""``pna_aggregate``: the PNA neighbourhood aggregation as one call into libpna_sm90.so.
 
 Replaces, for one layer call, the reference sequence (models/pytorch_geometric/pna.py:152-159 / :242-249):
 ``index_select`` of x_j, six ``scatter_add`` + ``scatter_min`` + ``scatter_max`` + ``degree`` passes over an
@@ -45,9 +45,9 @@ DYNAMIC_TAIL_MIN_PARTITION_COST = 256
 
 def _dynamic_tail(csr: CSRGraph) -> bool:
     """Hand the last 30 % of the row partitions out dynamically (pna_agg_t.work_counter)?  Every grab restarts the warp's
-    gather ring (~6 us of serial latency: counter, partition bounds, first sources, first rows), so it pays only when a
-    partition is much more work than that: config-5 share (420 slots+12*rows per partition) 3.30 -> 2.70 ms, config 2
-    (49 per partition) 0.271 -> 0.354 ms.  PNA_B200_DYNAMIC_TAIL=0/1 overrides."""
+    gather ring (serial latency: counter, partition bounds, first sources, first rows), so it pays only when a
+    partition is much more work than that: the config-5 share (420 slots+12*rows per partition) gains, config 2 (49 per
+    partition) loses.  PNA_B200_DYNAMIC_TAIL=0/1 overrides."""
     env = os.environ.get("PNA_B200_DYNAMIC_TAIL")
     if env is not None:
         return env != "0"
@@ -88,7 +88,7 @@ def aggregate_forward(gathered: torch.Tensor, csr: CSRGraph, aggregators: Names,
     if not gathered.is_cuda:
         raise ValueError("pna_b200 kernels run on CUDA tensors only; there is no CPU fallback")
     if gathered.dtype not in _DTYPES:
-        raise TypeError(f"unsupported dtype {gathered.dtype}; libpna_sm100 takes float32 and bfloat16")
+        raise TypeError(f"unsupported dtype {gathered.dtype}; libpna_sm90 takes float32 and bfloat16")
     dev = gathered.device
     if csr.device != dev:
         raise ValueError(f"CSR lives on {csr.device}, features on {dev}")
@@ -251,9 +251,8 @@ def _round_up(n: int, m: int) -> int:
 def backward_mode() -> str:
     """Which backward runs for gathered rows: "atomic" (default) = ``pna_aggregate_bwd``, one call, a vector atomic per edge and
     feature chunk; ``PNA_B200_BWD=coef`` = per-destination coefficient rows (``pna_aggregate_bwd_coef``), their sums over the
-    transposed graph through the forward kernels, ``pna_aggregate_bwd_combine`` -- atomics only for min / max.  Measured
-    (profiles/r02_backward_ab.json): config 2 1.12 ms atomic vs 1.30 ms coef; config-5 share (hot source rows) 50.2 vs 26.6 ms,
-    but regrouping sum_i (c0_i + c1_i x_j) into sum_i c0_i + x_j sum_i c1_i cancels badly where many rows have var ~ 0
+    transposed graph through the forward kernels, ``pna_aggregate_bwd_combine`` -- atomics only for min / max.  The
+    coefficient path avoids the atomics that contend on hot source rows (power-law graphs), but regrouping sum_i (c0_i + c1_i x_j) into sum_i c0_i + x_j sum_i c1_i cancels badly where many rows have var ~ 0
     (2.6x the fp32 error of the per-edge evaluation on a power-law multigraph), so it stays opt-in."""
     return "coef" if os.environ.get("PNA_B200_BWD", "atomic") == "coef" else "atomic"
 
@@ -296,7 +295,7 @@ def pna_aggregate(gathered: torch.Tensor, csr: CSRGraph, aggregators: Names, sca
                   self_feat: Optional[torch.Tensor] = None, self_divided: bool = True,
                   messages_in_csr_order: bool = False, zero_isolated: bool = False, relu_var: bool = False,
                   scaler_degree: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """Differentiable PNA aggregation (forward = one libpna_sm100 call).  See :func:`aggregate_forward`."""
+    """Differentiable PNA aggregation (forward = one libpna_sm90 call).  See :func:`aggregate_forward`."""
     needs_grad = torch.is_grad_enabled() and any(
         t is not None and t.requires_grad for t in (gathered, row_bias, self_feat))
     if not needs_grad:

@@ -1,4 +1,4 @@
-// Shared helpers for libpna_sm100.so (sm_100a only).
+// Shared helpers for libpna_sm90.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -7,8 +7,8 @@
 #include <stdarg.h>
 #include "../../include/pna_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libpna_sm100 is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libpna_sm90 is written for sm_90a (H100) only"
 #endif
 
 namespace pna {
@@ -83,7 +83,7 @@ __device__ __forceinline__ DegScales deg_scales(int deg, float avg_log, float av
 // re-read by this library, so it is stored with the streaming (evict-first) policy to keep source rows in L2.
 
 // How the [N, S*A*F] result leaves the SM.  0: st.global.cs (streaming, evict-first) -- the default; 1: plain st.global;
-// 2: st.global.cg; 3: st.global.wt.  A build-time knob for experiments (tools/exp/build_variant.sh).
+// 2: st.global.cg; 3: st.global.wt.  A build-time knob for experiments (nvcc -DPNA_STORE_MODE=n).
 #ifndef PNA_STORE_MODE
 #define PNA_STORE_MODE 0
 #endif

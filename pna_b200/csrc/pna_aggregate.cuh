@@ -1,6 +1,6 @@
 // Device-side building blocks of the PNA aggregation (forward).
 //
-// Work decomposition (B200-first, not a translation of torch_scatter's atomics):
+// Work decomposition (GPU-first, not a translation of torch_scatter's atomics):
 //   * destination rows are independent; a row is owned by a group of G lanes (G = 1..32, a power of two),
 //     32/G rows per warp.  Lanes map to FEATURE columns: lane g owns the 16-byte chunks g, g+G, .. (K of them), so
 //     every gathered neighbour row is read as fully coalesced 128-bit loads and NO cross-lane reduction is needed;
@@ -82,33 +82,14 @@ using CfgMeanMaxMinStd = CfgStatic<4, (1u) | (3u << 4) | (2u << 8) | (5u << 12),
 using CfgMeanMaxMinStdId = CfgStatic<4, (1u) | (3u << 4) | (2u << 8) | (5u << 12), 1, 0u>;
 using CfgMeanMinMaxStd = CfgStatic<4, (1u) | (2u << 4) | (3u << 8) | (5u << 12), 3, (0u) | (1u << 4) | (2u << 8)>;
 
-// ---- sm_100 packed fp32 arithmetic (FADD2 / FMUL2: two IEEE-rounded fp32 operations per issue slot) and the 3-input
-// FMNMX3.  Same roundings as the scalar forms -- mul.rn / add.rn are never contracted into an FMA -- so the
-// accumulation stays bit-identical to the reference's "sum += m; sumsq += m*m" sequence while the issue-slot cost of
-// one neighbour row drops from 20 to 10 instructions per 4 features.
-__device__ __forceinline__ float2 add2_rn(float2 a, float2 b) {
-  unsigned long long ra = *reinterpret_cast<unsigned long long*>(&a), rb = *reinterpret_cast<unsigned long long*>(&b), rd;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(ra), "l"(rb));
-  return *reinterpret_cast<float2*>(&rd);
-}
-__device__ __forceinline__ float2 mul2_rn(float2 a, float2 b) {
-  unsigned long long ra = *reinterpret_cast<unsigned long long*>(&a), rb = *reinterpret_cast<unsigned long long*>(&b), rd;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(ra), "l"(rb));
-  return *reinterpret_cast<float2*>(&rd);
-}
-// m*m per component with SCALAR multiplies: ptxas contracts mul.rn.f32x2 feeding add.rn.f32x2 into FFMA2 even with
-// -fmad=false, which would skip the rounding of the product that the reference's "src * src" performs.
+// ---- fp32 pair arithmetic.  Hopper has no packed fp32 add/multiply, so a pair is two IEEE-rounded scalar operations;
+// __fadd_rn / __fmul_rn are never contracted into an FMA, so the accumulation stays bit-identical to the reference's
+// "sum += m; sumsq += m*m" sequence (the product is rounded before it is added).
+__device__ __forceinline__ float2 add2_rn(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 mul2_rn(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 sqr2(float2 m) { return make_float2(__fmul_rn(m.x, m.x), __fmul_rn(m.y, m.y)); }
-__device__ __forceinline__ float min3f(float a, float b, float c) {
-  float d;
-  asm("min.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
-__device__ __forceinline__ float max3f(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
+__device__ __forceinline__ float min3f(float a, float b, float c) { return fminf(fminf(a, b), c); }
+__device__ __forceinline__ float max3f(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 
 template <int VEC>
 struct Acc {

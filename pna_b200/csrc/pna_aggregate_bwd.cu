@@ -12,7 +12,7 @@
 // chunk by three small kernels (statistics, coefficients, scatter), like the forward.
 //
 // pna_aggregate_bwd_coef (gathered rows, col != NULL): pass C and its one vector atomic per (slot, feature chunk) are what
-// bound the kernel above (REDG issue rate, ~0.9 TB/s of atomic traffic on the chip).  Per SOURCE row j the same gradient is
+// bound the kernel above (the issue rate of the REDG atomics).  Per SOURCE row j the same gradient is
 //   grad_gathered[j] = sum_{i <- j} (c0_i + c1_i * bias_i)  +  gathered[j] * sum_{i <- j} c1_i  +  routed min / max terms,
 // so this entry point stops after the coefficients: it writes the row [c0' | c1] per destination, routes min / max with ONE
 // scalar atomic per (row, feature) and writes grad_row_bias in closed form (deg * c0 + c1 * sum_m + gmin + gmax).  The two
@@ -569,8 +569,11 @@ extern "C" int pna_aggregate_bwd_combine(const float* coef_sums, int64_t ld_sums
               "pna_aggregate_bwd_combine: row pitch too small");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long total = n_src * (long long)n_feat;
+  int dev = 0, sms = 0;
+  PNA_CUDA_TRY(cudaGetDevice(&dev));
+  PNA_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;      // grid-stride: 16 CTAs of 256 threads per SM
+  if (blocks > sms * 8LL) blocks = sms * 8LL;    // grid-stride: 8 CTAs of 256 threads fill an SM (2048 threads)
   if (dtype == PNA_F32)
     k_bwd_combine<float><<<(unsigned)blocks, 256, 0, st>>>(coef_sums, ld_sums, c1_column, static_cast<const float*>(gathered),
                                                            ld_gathered, grad_gathered, ld_grad_gathered, n_src, n_feat);

@@ -320,9 +320,8 @@ struct StreamGeom {
 // 16-byte async copy global -> shared (LDGSTS, L2-only caching) with an L2 eviction-priority hint
 // L1 = true: the copy allocates in L1 (cp.async.ca).  A source row that many destinations of the same SM gather (power-law
 // graphs: a handful of rows receive a third of all gathers) is then served by the SM's own L1 instead of the few L2 slices
-// that hold its lines -- their bandwidth (about 1 TB/s for a 1 KB row) is what bounds such graphs otherwise: config-5 share
-// 4.57 -> 3.34 ms.  For graphs without hot sources the L1 detour costs (config 2: 0.277 -> 0.293 ms), hence a mode the
-// caller selects (PNA_FLAG_GATHER_L1), not a default.
+// that hold its lines -- their bandwidth is what bounds such graphs otherwise.  For graphs without hot sources the L1
+// detour costs time, hence a mode the caller selects (PNA_FLAG_GATHER_L1), not a default.
 template <bool L1 = false>
 __device__ __forceinline__ void cp_async16(unsigned dst, const void* src, unsigned long long policy) {
   if constexpr (L1)
@@ -965,7 +964,7 @@ static int launch_config(const KParams& p_in, cudaStream_t st) {
   do {                                                                                                             \
     constexpr size_t smem = StreamGeom<T, VEC, K, DEPTH>::kSmem;                                                   \
     auto kern = k_rows_stream<T, VEC, K, CFG, B, DEPTH, FOLD, L1>;                                                     \
-    static int resident = 0;  /* CTAs of this kernel that fit the device (all B200s alike) */                     \
+    static int resident = 0;  /* CTAs of this kernel that fit the device (every device of a process alike) */                \
     if (resident == 0) {                                                                                           \
       if (smem > 48 * 1024) PNA_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
       int dev = 0, sms = 0, nb = 0;                                                                                \

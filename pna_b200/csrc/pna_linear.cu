@@ -1,20 +1,23 @@
-// pna_linear_fwd: Y[N, O] = A[N, K] . W[O, K]^T + b in fp32 accuracy on the 5th-generation tensor cores.
+// pna_linear_fwd: Y[N, O] = A[N, K] . W[O, K]^T + b in fp32 accuracy on the Hopper tensor cores (wgmma).
 //
 // This is the first dense linear of the post-aggregation MLP (reference models/pytorch_geometric/pna.py:222-227,
 // post_nn[0]; models/dgl/pna_layer.py:31 posttrans), the one place of the PNA layer where tensor cores apply
 // (north_star: "the post-MLP uses tensor cores only for its dense linear").  The 1e-5 parity bar rules out plain TF32
 // (10-bit mantissa); every operand is therefore split  x = hi + lo  (hi = top 19 bits, lo = x - hi, exact) and three
-// tcgen05.mma kind::tf32 products are accumulated in TMEM:  hi.hi + hi.lo + lo.hi  (the dropped lo.lo term is 2^-22).
+// wgmma tf32 products are accumulated in registers:  hi.hi + hi.lo + lo.hi  (the dropped lo.lo term is 2^-22).
 //
-// One CTA per 128-row tile, 10 warps, 3-stage mbarrier ring of {A hi, A lo, W hi, W lo} tiles:
-//   warps 0-7  A loaders: coalesced 128-bit loads issued four K blocks ahead, split hi / lo (cvt.rna.tf32: an unbiased
-//              split -- truncation accumulates its one-sided error linearly in K) and stored into the 128-byte-swizzled
-//              K-major layout UMMA reads (the operand has to pass through registers for the split, so no TMA here).
-//              Warps 0-3 are afterwards the epilogue: tcgen05.ld the accumulator, add the bias, store.
-//   warp 8     allocates TMEM and issues the MMAs from one elected lane: 12 per 32-wide K block
-//              (4 K-steps x 3 products); tcgen05.commit releases the stage / signals the epilogue.
-//   warp 9     W producer: the weight is pre-split once per call into the exact swizzled shared-memory image of every
-//              K block, so a W tile is one contiguous cp.async.bulk (TMA 1-D) completing on the stage's mbarrier.
+// Two warpgroups (256 threads), 3-stage (2 for O = 256) mbarrier ring of {A hi, A lo, W hi, W lo} tiles:
+//   all warps  load A with coalesced 128-bit loads issued ahead, split hi / lo (cvt.rna.tf32: an unbiased split --
+//              truncation accumulates its one-sided error linearly in K) and store into the 128-byte-swizzled K-major
+//              layout wgmma reads (the operand has to pass through registers for the split, so no TMA here).  The same
+//              warps then issue the stage's wgmmas (12 per 32-wide K block: 4 K-steps x 3 products) and, one stage
+//              later, release it.  Warpgroup g owns a 64 x min(O, 128) block of the CTA's output: rows 64g.. of a
+//              128-row tile for O <= 128, columns 128g.. of a 64-row tile for O = 256 (two fp32 accumulators of
+//              64 x 256 would not fit the register file).  The epilogue adds the accumulators and the bias and stores.
+//   thread 0   also issues the W tiles: the weight is pre-split once per call into the exact swizzled shared-memory image
+//              of every K block, so a W tile is one contiguous cp.async.bulk (TMA 1-D) completing on the stage's mbarrier;
+//              the tile of step t + kSt is requested as soon as step t has released its stage.  (A separate producer
+//              warp would lower the per-thread register budget below the two accumulators.)
 //
 // Scaled ("compact") mode -- pna_linear_scaled_fwd.  The reference's post-MLP input is cat_s(c_s(i) * agg_i) over the
 // degree scalers s (pna.py:247-249): S copies of the same [N, A*F] aggregate, each multiplied by a per-row factor.  In
@@ -26,11 +29,10 @@
 
 namespace pna {
 
-constexpr int kLinM = 128;          // rows per CTA (UMMA_M)
 constexpr int kLinBK = 32;          // fp32 per K block = one 128-byte swizzle row
-constexpr int lin_stages(int o) { return o <= 128 ? 3 : 2; }   // 64 KB (O=128) / 96 KB (O=256) per stage
-constexpr int kLinLoaders = 256;    // warps 0-7: A loaders (warps 0-3 are also the epilogue)
-constexpr int kLinThreads = kLinLoaders + 64;   // + warp 8: MMA issuer, warp 9: W tile producer (bulk copies)
+constexpr int lin_rows(int o) { return o <= 128 ? 128 : 64; }      // rows per CTA
+constexpr int lin_stages(int o) { return o <= 128 ? 3 : 2; }       // 48 / 64 / 80 KB per stage (O = 64 / 128 / 256)
+constexpr int kLinThreads = 256;    // two warpgroups: A loaders and MMA issuers
 
 __device__ __forceinline__ unsigned lin_smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void lin_mbar_init(unsigned bar, unsigned count) {
@@ -64,37 +66,64 @@ __device__ __forceinline__ float lin_tf32(float x) {
   return __uint_as_float(r);
 }
 
-// shared-memory matrix descriptor: K-major, SWIZZLE_128B, rows of 128 bytes, 8-row groups 1024 bytes apart
+// wgmma shared-memory matrix descriptor: K-major, SWIZZLE_128B, rows of 128 bytes, 8-row groups 1024 bytes apart.
+// A K step inside the 128-byte row advances the start address (the swizzle is applied to the computed addresses).
 __device__ __forceinline__ unsigned long long lin_desc(unsigned smem_addr) {
   unsigned long long d = 0;
   d |= (unsigned long long)((smem_addr & 0x3ffffu) >> 4);        // start address, bits [0,14)
   d |= (unsigned long long)1 << 16;                               // leading byte offset (unused for swizzled K-major)
   d |= (unsigned long long)(1024 >> 4) << 32;                     // stride byte offset: 8 rows x 128 B
-  d |= (unsigned long long)1 << 46;                               // descriptor version (Blackwell)
-  d |= (unsigned long long)2 << 61;                               // SWIZZLE_128B
+  d |= (unsigned long long)1 << 62;                               // SWIZZLE_128B
   return d;
 }
 
-__device__ __forceinline__ void lin_mma_tf32(unsigned tmem_d, unsigned long long adesc, unsigned long long bdesc, unsigned idesc,
-                                             unsigned accumulate) {
+#define LIN_F4(a, i) "+f"(a[i]), "+f"(a[i + 1]), "+f"(a[i + 2]), "+f"(a[i + 3])
+#define LIN_F16(a, i) LIN_F4(a, i), LIN_F4(a, i + 4), LIN_F4(a, i + 8), LIN_F4(a, i + 12)
+
+// D[64 x N] += A[64 x 8] . B[N x 8]^T, tf32 operands from shared memory, fp32 accumulator in registers (N/2 per thread:
+// register 4j + q of lane l holds row l/4 + 8 (q/2) of the warp's 16 rows, column 8j + 2 (l%4) + q%2)
+template <int N>
+__device__ __forceinline__ void lin_wgmma(float (&d)[N / 2], unsigned long long adesc, unsigned long long bdesc);
+template <>
+__device__ __forceinline__ void lin_wgmma<64>(float (&d)[32], unsigned long long adesc, unsigned long long bdesc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+      "}, %32, %33, p, 1, 1;\n\t}"
+      : LIN_F16(d, 0), LIN_F16(d, 16)
+      : "l"(adesc), "l"(bdesc));
+}
+template <>
+__device__ __forceinline__ void lin_wgmma<128>(float (&d)[64], unsigned long long adesc, unsigned long long bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1;\n\t}"
+      : LIN_F16(d, 0), LIN_F16(d, 16), LIN_F16(d, 32), LIN_F16(d, 48)
+      : "l"(adesc), "l"(bdesc));
+}
+// keeps the compiler from moving accumulator registers across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void lin_fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 // byte offset of 16-byte unit j of row r inside a [rows][128 B] tile with the 128-byte swizzle (unit ^= row % 8)
 __host__ __device__ __forceinline__ unsigned lin_swz(int r, int j) { return (unsigned)(r * 128 + ((j ^ (r & 7)) << 4)); }
 
-template <int O>   // output width = UMMA_N, a multiple of 16 up to 256
+template <int O>   // output width: 64, 128 or 256
 struct LinSmem {
+  static constexpr int kM = lin_rows(O);
   static constexpr int kSt = lin_stages(O);
-  // TMEM accumulators: kMain for hi.hi (K blocks dealt round-robin: fewer truncating accumulation steps and a smaller
-  // running sum per accumulator) + 1 for the two cross terms
-  static constexpr int kMain = (3 * O <= 512) ? 2 : 1;
-  static constexpr unsigned kCols = (kMain + 1) * O <= 64 ? 64 : (kMain + 1) * O <= 128 ? 128 : (kMain + 1) * O <= 256 ? 256 : 512;
-  static constexpr int kATile = kLinM * 128;                  // bytes of one A hi (or lo) stage
+  static constexpr int kN = O <= 128 ? O : 128;               // output columns per warpgroup
+  static constexpr int kATile = kM * 128;                     // bytes of one A hi (or lo) stage
   static constexpr int kWTile = O * 128;
   static constexpr int kStage = 2 * kATile + 2 * kWTile;
   static constexpr size_t kBytes = 1024 /*align slack*/ + (size_t)kSt * kStage + 256;
@@ -107,41 +136,52 @@ __global__ void __launch_bounds__(kLinThreads, 1)
 k_linear_3xtf32(const float* __restrict__ A, long long lda, const float* __restrict__ row_scale, int n_rep,
                 const float* __restrict__ Wimg, const float* __restrict__ bias, float* __restrict__ Y, long long ldy, long long N,
                 int K) {
-  constexpr int kSt = LinSmem<O>::kSt;
+  constexpr int kSt = LinSmem<O>::kSt, kM = LinSmem<O>::kM, kN = LinSmem<O>::kN;
   extern __shared__ unsigned char lin_raw[];
   const unsigned base = (lin_smem_u32(lin_raw) + 1023u) & ~1023u;          // swizzle atoms need 1024-byte alignment
   unsigned char* gbase = lin_raw + (base - lin_smem_u32(lin_raw));
-  const unsigned bars = base + kSt * LinSmem<O>::kStage;                    // full[kSt], empty[kSt], tmem_full, tmem slot
+  const unsigned bars = base + kSt * LinSmem<O>::kStage;                    // full[kSt], empty[kSt]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const long long row0 = (long long)blockIdx.x * kLinM;
+  const long long row0 = (long long)blockIdx.x * kM;
   const int n_kb = K / kLinBK;          // K blocks of A (compact width)
   const int n_it = n_kb * n_rep;        // pipeline steps = K blocks of W (n_rep == 1 without row scales)
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kSt; ++s) {
-      lin_mbar_init(bars + 8 * s, kLinLoaders / 32 + 1);    // full: one arrive per A-loader warp + the W producer (with tx bytes)
-      lin_mbar_init(bars + 8 * (kSt + s), 1);               // empty: tcgen05.commit
+      lin_mbar_init(bars + 8 * s, kLinThreads / 32 + 1);    // full: one arrive per warp + the W request (with tx bytes)
+      lin_mbar_init(bars + 8 * (kSt + s), kLinThreads / 32); // empty: one arrive per warp once its MMAs have read the stage
     }
-    lin_mbar_init(bars + 8 * (2 * kSt), 1);                 // accumulator ready
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 8) {   // TMEM: O columns (power of two >= 32)
-    constexpr unsigned cols = LinSmem<O>::kCols;
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(bars + 8 * (2 * kSt + 1)), "n"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+  // W tiles of pipeline step t: two bulk copies (hi, lo images) into stage t % kSt
+  auto request_w = [&](int t) {
+    const int sw = t % kSt;
+    const int kb = (t % n_rep) * n_kb + t / n_rep;         // weight K block of (compact block t / n_rep, scaler t % n_rep)
+    const unsigned st = base + sw * LinSmem<O>::kStage + 2 * LinSmem<O>::kATile;
+    lin_mbar_expect_tx(bars + 8 * sw, 2u * LinSmem<O>::kWTile);
+    const float* img = Wimg + (long long)kb * (2 * O * kLinBK);
+    lin_bulk_g2s(st, img, LinSmem<O>::kWTile, bars + 8 * sw);
+    lin_bulk_g2s(st + LinSmem<O>::kWTile, img + O * kLinBK, LinSmem<O>::kWTile, bars + 8 * sw);
+  };
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const unsigned tmem = *reinterpret_cast<volatile unsigned*>(gbase + kSt * LinSmem<O>::kStage + 8 * (2 * kSt + 1));
+  if (threadIdx.x == 0)
+    for (int t = 0; t < kSt && t < n_it; ++t) request_w(t);   // every stage starts empty
 
-  if (warp < 8) {
-    // ---------------- A loaders: LDG two K blocks ahead -> split hi/lo -> swizzled STS ----------------
+  {
+    // ---------------- A loaders + MMA issuers: LDG ahead -> split hi/lo -> swizzled STS -> wgmma ----------------
     const int tid = threadIdx.x;                            // 0..255
     const int j = tid & 7;                                  // 16-byte unit inside the 128-byte K block row
     const int r_in = tid >> 3;                              // 0..31: row inside a 32-row slab
-    constexpr int kSlabs = kLinM / 32;                      // 4
-    constexpr int kAhead = 4;                               // K blocks of A kept in flight per thread (16 x 16 B)
+    constexpr int kSlabs = kM / 32;                         // 4 (O <= 128) or 2 (O = 256)
+    constexpr int kAhead = 8 / kSlabs;                      // K blocks of A kept in flight per thread (8 x 16 B)
+    const int wg = warp >> 2;                               // warpgroup: which 64 x kN block of the output it owns
+    const unsigned a_off = O <= 128 ? (unsigned)(wg * 64 * 128) : 0u;
+    const unsigned w_off = O <= 128 ? 0u : (unsigned)(wg * kN * 128);
+    // the tensor core adds into fp32 with truncation, a bias that grows with the number of accumulation steps times the
+    // magnitude of the running sum: the two small cross terms (2^-11 of the main product) get their own accumulator
+    float acc[kN / 2], corr[kN / 2];
+#pragma unroll
+    for (int i = 0; i < kN / 2; ++i) { acc[i] = 0.f; corr[i] = 0.f; }
     float4 pre[kAhead][kSlabs];
     auto fetch = [&](int kb, float4 (&dst)[kSlabs]) {
 #pragma unroll
@@ -155,6 +195,8 @@ k_linear_3xtf32(const float* __restrict__ A, long long lda, const float* __restr
     for (int u = 0; u < kAhead; ++u) fetch(u, pre[u]);
     unsigned phase = 0;
     int s = 0;                                              // ring stage of the next pipeline step
+    int prev = -1;                                          // stage whose MMAs are still in flight
+    int it = 0;                                             // pipeline step
     for (int kb0 = 0; kb0 < n_kb; kb0 += kAhead) {
 #pragma unroll
       for (int u = 0; u < kAhead; ++u) {                    // unrolled so that pre[u] stays in registers
@@ -191,104 +233,52 @@ k_linear_3xtf32(const float* __restrict__ A, long long lda, const float* __restr
           asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // generic-proxy stores -> visible to the MMA (async proxy)
           __syncwarp();
           if (lane == 0) lin_mbar_arrive(bars + 8 * s);
+          lin_mbar_wait(bars + 8 * s, phase);               // every warp's A rows and the W tiles have landed
+          const unsigned sa = base + s * LinSmem<O>::kStage;
+          const unsigned a_hi = sa + a_off, a_lo = sa + LinSmem<O>::kATile + a_off;
+          const unsigned w_hi = sa + 2 * LinSmem<O>::kATile + w_off, w_lo = w_hi + LinSmem<O>::kWTile;
+          lin_fence_acc(acc); lin_fence_acc(corr);
+          asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll
+          for (int ks = 0; ks < kLinBK / 8; ++ks) {         // K = 8 tf32 = 32 bytes along the swizzled row
+            const unsigned ko = ks * 32;
+            lin_wgmma<kN>(corr, lin_desc(a_hi + ko), lin_desc(w_lo + ko));
+            lin_wgmma<kN>(corr, lin_desc(a_lo + ko), lin_desc(w_hi + ko));
+            lin_wgmma<kN>(acc, lin_desc(a_hi + ko), lin_desc(w_hi + ko));
+          }
+          asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+          asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");     // the previous step's MMAs are done
+          lin_fence_acc(acc); lin_fence_acc(corr);
+          if (prev >= 0) {
+            if (lane == 0) lin_mbar_arrive(bars + 8 * (kSt + prev));
+            const int t = it - 1 + kSt;                     // the next step that uses the released stage
+            if (threadIdx.x == 0 && t < n_it) {
+              lin_mbar_wait(bars + 8 * (kSt + prev), ((unsigned)((it - 1) / kSt)) & 1u);   // every warp is done with it
+              request_w(t);
+            }
+            __syncwarp();
+          }
+          prev = s;
+          ++it;
           if (++s == kSt) { s = 0; phase ^= 1; }
         }
       }
     }
-    if (warp < 4) {
-      // ---------------- epilogue ----------------
-      lin_mbar_wait(bars + 8 * (2 * kSt), 0);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const long long row = row0 + warp * 32 + lane;        // TMEM lane = accumulator row; warp w owns lanes 32w..32w+31
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+    lin_fence_acc(acc); lin_fence_acc(corr);
+    // ---------------- epilogue: (main + cross terms) + bias, two adjacent columns per store ----------------
+    const int wr = (warp & 3) * 16 + (lane >> 2);           // row of the warpgroup's 64 for registers 4j, 4j + 1
+    const long long r_lo = row0 + (O <= 128 ? wg * 64 : 0) + wr, r_hi = r_lo + 8;
 #pragma unroll
-      for (int c0 = 0; c0 < O; c0 += 16) {
-        unsigned v[16];
-        const unsigned taddr = tmem + ((unsigned)(warp * 32) << 16) + (unsigned)c0;
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-              "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-            : "r"(taddr));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int acc = 1; acc <= LinSmem<O>::kMain; ++acc) {     // the other main accumulator(s) (only if K reached them) + cross terms
-          if (acc < LinSmem<O>::kMain && n_it <= acc) continue;
-          unsigned c[16];
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-              : "=r"(c[0]), "=r"(c[1]), "=r"(c[2]), "=r"(c[3]), "=r"(c[4]), "=r"(c[5]), "=r"(c[6]), "=r"(c[7]), "=r"(c[8]), "=r"(c[9]),
-                "=r"(c[10]), "=r"(c[11]), "=r"(c[12]), "=r"(c[13]), "=r"(c[14]), "=r"(c[15])
-              : "r"(taddr + acc * O));
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) + __uint_as_float(c[i]));
-        }
-        if (row < N) {
-          float* yr = Y + row * ldy + c0;
-#pragma unroll
-          for (int i = 0; i < 16; i += 4) {
-            float4 o;
-            o.x = __uint_as_float(v[i]) + (bias ? __ldg(bias + c0 + i) : 0.f);
-            o.y = __uint_as_float(v[i + 1]) + (bias ? __ldg(bias + c0 + i + 1) : 0.f);
-            o.z = __uint_as_float(v[i + 2]) + (bias ? __ldg(bias + c0 + i + 2) : 0.f);
-            o.w = __uint_as_float(v[i + 3]) + (bias ? __ldg(bias + c0 + i + 3) : 0.f);
-            *reinterpret_cast<float4*>(yr + i) = o;
-          }
-        }
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    for (int jj = 0; jj < kN / 8; ++jj) {
+      const int c = (O <= 128 ? 0 : wg * kN) + jj * 8 + 2 * (lane & 3);
+      const float b0 = bias ? __ldg(bias + c) : 0.f, b1 = bias ? __ldg(bias + c + 1) : 0.f;
+      if (r_lo < N)
+        *reinterpret_cast<float2*>(Y + r_lo * ldy + c) = make_float2((acc[4 * jj] + corr[4 * jj]) + b0, (acc[4 * jj + 1] + corr[4 * jj + 1]) + b1);
+      if (r_hi < N)
+        *reinterpret_cast<float2*>(Y + r_hi * ldy + c) =
+            make_float2((acc[4 * jj + 2] + corr[4 * jj + 2]) + b0, (acc[4 * jj + 3] + corr[4 * jj + 3]) + b1);
     }
-  } else if (warp == 8) {
-    // ---------------- MMA issuer ----------------
-    constexpr unsigned idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((unsigned)(O >> 3) << 17) | ((unsigned)(kLinM >> 4) << 24);
-    unsigned phase = 0;
-    for (int kb = 0; kb < n_it; ++kb) {                     // kb: pipeline step (= K block of the scaled operand)
-      const int s = kb % kSt;
-      lin_mbar_wait(bars + 8 * s, phase);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (lane == 0) {
-        const unsigned st = base + s * LinSmem<O>::kStage;
-        const unsigned a_hi = st, a_lo = st + LinSmem<O>::kATile, w_hi = st + 2 * LinSmem<O>::kATile,
-                       w_lo = w_hi + LinSmem<O>::kWTile;
-#pragma unroll
-        for (int ks = 0; ks < kLinBK / 8; ++ks) {            // UMMA_K = 8 tf32 = 32 bytes along the swizzled row
-          const unsigned ko = ks * 32;
-          // the tensor core adds into fp32 with truncation, a bias that grows with the number of accumulation steps
-          // times the magnitude of the running sum: the two small cross terms (2^-11 of the main product) get their own
-          // accumulator, and the main product alternates between kMain accumulators
-          constexpr int kMain = LinSmem<O>::kMain;
-          const unsigned corr = tmem + kMain * O, mainacc = tmem + (kb % kMain) * O;
-          lin_mma_tf32(corr, lin_desc(a_hi + ko), lin_desc(w_lo + ko), idesc, (kb | ks) ? 1u : 0u);
-          lin_mma_tf32(corr, lin_desc(a_lo + ko), lin_desc(w_hi + ko), idesc, 1u);
-          lin_mma_tf32(mainacc, lin_desc(a_hi + ko), lin_desc(w_hi + ko), idesc, (kb >= kMain || ks) ? 1u : 0u);
-        }
-        // release the stage when these MMAs have read it; after the last block also publish the accumulator
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bars + 8 * (kSt + s)) : "memory");
-        if (kb == n_it - 1)
-          asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bars + 8 * (2 * kSt)) : "memory");
-      }
-      __syncwarp();
-      if (s == kSt - 1) phase ^= 1;
-    }
-  } else if (warp == 9 && lane == 0) {
-    // ---------------- W tile producer: two bulk copies (hi, lo images) per K block ----------------
-    unsigned phase = 0;
-    for (int it = 0; it < n_it; ++it) {
-      const int s = it % kSt;
-      const int kb = (it % n_rep) * n_kb + it / n_rep;     // weight K block of (compact block it / n_rep, scaler it % n_rep)
-      lin_mbar_wait(bars + 8 * (kSt + s), phase ^ 1);
-      const unsigned st = base + s * LinSmem<O>::kStage + 2 * LinSmem<O>::kATile;
-      lin_mbar_expect_tx(bars + 8 * s, 2u * LinSmem<O>::kWTile);
-      const float* img = Wimg + (long long)kb * (2 * O * kLinBK);
-      lin_bulk_g2s(st, img, LinSmem<O>::kWTile, bars + 8 * s);
-      lin_bulk_g2s(st + LinSmem<O>::kWTile, img + O * kLinBK, LinSmem<O>::kWTile, bars + 8 * s);
-      if (s == kSt - 1) phase ^= 1;
-    }
-  }
-  __syncthreads();
-  if (warp == 8) {
-    constexpr unsigned cols = LinSmem<O>::kCols;
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(cols) : "memory");
   }
 }
 
@@ -320,7 +310,7 @@ static int launch_linear(const float* A, long long lda, const float* row_scale, 
     PNA_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LinSmem<O>::kBytes));
     attr_set = true;
   }
-  const long long grid = (N + kLinM - 1) / kLinM;
+  const long long grid = (N + LinSmem<O>::kM - 1) / LinSmem<O>::kM;
   kern<<<(unsigned)grid, kLinThreads, LinSmem<O>::kBytes, st>>>(A, lda, row_scale, n_rep, Wimg, bias, Y, ldy, N, K);
   PNA_CUDA_TRY(cudaGetLastError());
   return PNA_OK;

@@ -48,7 +48,7 @@ extern "C" const char* pna_last_error(void) { return g_err; }
 extern "C" int pna_query(int what) {
   switch (what) {
     case PNA_QUERY_ABI_VERSION: return PNA_ABI_VERSION;
-    case PNA_QUERY_SM_ARCH: return 100;
+    case PNA_QUERY_SM_ARCH: return 90;
     case PNA_QUERY_DEFAULT_SPLIT: return 256;
     case PNA_QUERY_DEFAULT_CHUNK: return 128;
     case PNA_QUERY_MAX_FEATURES: return 16384;

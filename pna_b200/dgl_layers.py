@@ -1,4 +1,4 @@
-"""DGL-signature PNA layers (reference ``models/dgl/pna_layer.py``) on the sm_100a aggregation kernel.
+"""DGL-signature PNA layers (reference ``models/dgl/pna_layer.py``) on the sm_90a aggregation kernel.
 
 Same constructors, same ``forward(g, h, e, snorm_n)`` / ``forward(g, h)``, same parameter names
 (``towers.{t}.pretrans.fully_connected.{k}.linear``, ``...posttrans...``, ``towers.{t}.batchnorm_h``,

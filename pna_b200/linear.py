@@ -1,4 +1,4 @@
-"""First dense linear of the post-aggregation MLP on the B200 tensor cores (``pna_linear_fwd``, 3xTF32 tcgen05).
+"""First dense linear of the post-aggregation MLP on the H100 tensor cores (``pna_linear_fwd``, 3xTF32 wgmma).
 
 ``post_linear(a, weight, bias)`` is ``torch.nn.functional.linear`` for the shapes the kernel takes
 (fp32, in_features % 32 == 0, out_features in {64, 128, 256}) and falls back to the library GEMM for every other shape --

@@ -1,4 +1,4 @@
-"""PyG-signature PNA layers backed by the sm_100a aggregation kernel.
+"""PyG-signature PNA layers backed by the sm_90a aggregation kernel.
 
 Drop-in for reference ``models/pytorch_geometric/pna.py``: same constructor arguments, same
 ``forward(x, edge_index, edge_attr=None)``, same parameter names (``pre_nns.{t}.{k}``, ``post_nns.{t}.{k}``,
@@ -108,7 +108,7 @@ class PNAConvSimple(Module):
     def _post(self, agg: Tensor, row_scale: Optional[Tensor], dtype) -> Tensor:
         """post_nn on (a row block of) the aggregated tensor; padding is absorbed by zero columns of the first Linear."""
         lin0 = self.post_nn[0]
-        # first Linear: tensor cores (3xTF32 tcgen05, pna_linear_fwd) when the shape allows, else the library GEMM
+        # first Linear: tensor cores (3xTF32 wgmma, pna_linear_fwd) when the shape allows, else the library GEMM
         if row_scale is not None:
             out = post_linear_scaled(agg, row_scale, self._first_weight(dtype), lin0.bias)
         else:

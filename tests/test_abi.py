@@ -24,7 +24,7 @@ def test_library_is_built_and_loads():
     assert os.path.exists(_lib.LIB_PATH), "run __graft_entry__.build()"
     L = _lib.lib()
     assert L.pna_query(_lib.QUERY_ABI_VERSION) == _lib.ABI_VERSION == 8
-    assert L.pna_query(_lib.QUERY_SM_ARCH) == 100
+    assert L.pna_query(_lib.QUERY_SM_ARCH) == 90
 
 
 def test_every_declared_symbol_is_exported():
@@ -40,11 +40,11 @@ def test_struct_layouts_match_the_header():
     assert _lib.query(_lib.QUERY_SIZEOF_AGG) == C.sizeof(_lib.AggStruct)
 
 
-def test_library_targets_sm_100a_only():
+def test_library_targets_sm_90a_only():
     import subprocess
     out = subprocess.run(["cuobjdump", "--list-elf", _lib.LIB_PATH], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_(\d+a?)", out))
-    assert archs == {"100a"}, archs
+    assert archs == {"90a"}, archs
 
 
 def test_queries_and_defaults_without_gpu():

@@ -1,6 +1,5 @@
 """Pin oracle/pna_oracle.py against outputs of the reference's own files (tests/golden, made by oracle/gen_golden.py)."""
 import math
-import os
 
 import pytest
 import torch
@@ -11,12 +10,32 @@ from conftest import load_golden
 SIMPLE = ["pyg_simple_f16", "pyg_simple_f64_hub", "pyg_simple_f75_const", "pyg_simple_allops"]
 CONV = ["pyg_conv_t1", "pyg_conv_t4_div", "pyg_conv_t5_rep", "pyg_conv_edge", "pyg_conv_pre2", "pyg_conv_multitask"]
 
+# The fixtures were made on one CPU; the oracle reruns the same torch ops on whatever CPU runs the suite.  Sums, min / max,
+# divisions and products are correctly rounded, so the columns built only from them are bit-reproducible on any host.
+# torch's vectorised CPU log and sqrt are not correctly rounded and take other code paths on CPUs with other instruction
+# sets: the std columns and the log-degree scalers agree to a few ulp.  Matrix products (pre- / post-MLP) are summed in a
+# BLAS-dependent order: what passes through them agrees to fp32 GEMM rounding.
+FEW_ULP = dict(rtol=1e-6, atol=1e-8)
+GEMM_TOL = dict(rtol=1e-5, atol=1e-5)
+
+
+def assert_aggregate_matches(got, want, aggregators, scalers):
+    """[N, S*A*F] aggregate (scaler-major): exact where only correctly rounded operations are involved, FEW_ULP elsewhere."""
+    S, A = len(scalers), len(aggregators)
+    g, w = got.view(got.size(0), S, A, -1), want.view(want.size(0), S, A, -1)
+    for si, sc in enumerate(scalers):
+        for ai, ag in enumerate(aggregators):
+            if sc in ("amplification", "attenuation") or ag == "std":
+                torch.testing.assert_close(g[:, si, ai], w[:, si, ai], **FEW_ULP)
+            else:
+                assert torch.equal(g[:, si, ai], w[:, si, ai]), (sc, ag)
+
 
 @pytest.mark.parametrize("name", SIMPLE)
 def test_simple_propagate_bit_exact(name):
     g = load_golden(name)
     agg = O.simple_propagate(g["x"], g["edge_index"], g["aggregators"], g["scalers"], g["avg_deg"])
-    assert torch.equal(agg, g["aggregate"])          # same torch ops in the same order -> bit identical
+    assert_aggregate_matches(agg, g["aggregate"], g["aggregators"], g["scalers"])    # same torch ops in the same order
     mine = O.avg_deg_from_histogram(g["deg"])
     assert mine["lin"] == g["avg_deg"]["lin"] and mine["log"] == g["avg_deg"]["log"]   # 'exp' overflows to nan for hubs
 
@@ -29,7 +48,7 @@ def test_simple_layer_forward(name):
     lay.load_state_dict(g["state_dict"])
     with torch.no_grad():
         out = lay(g["x"], g["edge_index"])
-    assert torch.equal(out, g["out"])
+    torch.testing.assert_close(out, g["out"], **GEMM_TOL)
 
 
 @pytest.mark.parametrize("name", CONV)
@@ -45,8 +64,17 @@ def test_conv_layer_forward(name):
     with torch.no_grad():
         agg = lay.propagate(xt, g["edge_index"], g["edge_attr"])
         out = lay(x, g["edge_index"], g["edge_attr"])
-    assert torch.equal(agg, g["aggregate"])
-    assert torch.equal(out, g["out"])
+    # messages come out of the pre-MLP's matrix products, so the aggregate too agrees to fp32 GEMM rounding -- except that
+    # sqrt(var + 1e-5) amplifies that rounding up to 158x where var ~ 0: the std columns are compared through their
+    # square, the variance, whose error is fp32 rounding of E[m^2]
+    S, A = len(g["scalers"]), len(g["aggregators"])
+    std_col = torch.zeros(S, A, agg.size(-1) // (S * A), dtype=torch.bool)
+    if "std" in g["aggregators"]:
+        std_col[:, g["aggregators"].index("std")] = True
+    std_col = std_col.flatten()
+    torch.testing.assert_close(agg[..., ~std_col], g["aggregate"][..., ~std_col], **GEMM_TOL)
+    torch.testing.assert_close(agg[..., std_col] ** 2, g["aggregate"][..., std_col] ** 2, rtol=1e-5, atol=1e-6)
+    torch.testing.assert_close(out, g["out"], **GEMM_TOL)
 
 
 @pytest.mark.parametrize("name", ["dgl_simple", "dgl_simple_var"])
@@ -54,7 +82,7 @@ def test_dgl_reduce_matches_reference_mailbox_reduce(name):
     g = load_golden(name)
     ei = g["edge_index"]
     agg = O.dgl_reduce(g["h"][ei[0]], None, ei[1], g["h"].size(0), g["aggregators"].split(), g["scalers"].split(), g["avg_d"])
-    assert torch.equal(agg, g["aggregate"])
+    assert_aggregate_matches(agg, g["aggregate"], g["aggregators"].split(), g["scalers"].split())
     # in-degree-0 rows are all zero in the DGL flavour, std columns included
     iso = torch.bincount(ei[1], minlength=g["h"].size(0)) == 0
     assert iso.any() and agg[iso].abs().max() == 0
@@ -120,23 +148,12 @@ def test_k3_analytic_rows():
     torch.testing.assert_close(out[1], torch.cat([base, base * amp, base * att]), rtol=1e-6, atol=1e-7)
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/models"), reason="reference checkout not on this machine")
 def test_live_reference_over_shims():
-    """In the authoring container, re-run the real reference file and compare with the oracle on fresh inputs."""
-    import subprocess, sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    code = (
-        "import torch\n"
-        "from models.pytorch_geometric.pna import PNAConvSimple\n"
-        "from oracle import pna_oracle as O\n"
-        "torch.manual_seed(5); n,e,f=300,2000,24\n"
-        "x=torch.randn(n,f); ei=torch.randint(0,n,(2,e)); deg=torch.bincount(torch.bincount(ei[1],minlength=n))\n"
-        "A=['mean','min','max','std']; S=['identity','amplification','attenuation']\n"
-        "c=PNAConvSimple(f,f,A,S,deg); r=c.propagate(ei,x=x,size=None)\n"
-        "assert torch.equal(r,O.simple_propagate(x,ei,A,S,c.avg_deg)); print('ok')\n")
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join([os.path.join(root, "oracle", "shims"), "/root/reference", root]))
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env, cwd=root)
-    assert r.returncode == 0 and "ok" in r.stdout, r.stderr
+    """The reference's own PNAConvSimple.propagate, run over oracle/shims on fresh random inputs and stored by
+    oracle/gen_golden.py --live, equals the oracle (bit for bit where the host's CPU kernels allow, see FEW_ULP)."""
+    g = load_golden("pyg_simple_live")
+    agg = O.simple_propagate(g["x"], g["edge_index"], g["aggregators"], g["scalers"], g["avg_deg"])
+    assert_aggregate_matches(agg, g["aggregate"], g["aggregators"], g["scalers"])
 
 
 def test_c_oracle_agrees_with_torch_oracle():

@@ -1,6 +1,6 @@
 """Time the aggregation on every BASELINE.json config shape that fits one GPU; parity-check a sample of rows.
 
-    python tools/config_sweep.py [--out profiles/r01_config_sweep.json]
+    python tools/config_sweep.py [--out sweep.json]
 Prints one line per config: N, E, F, dtype, ms, edges/s, B_min GB/s, fraction of the measured HBM peak."""
 import argparse, json, os, statistics, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -14,7 +14,7 @@ dev = torch.device("cuda:0")
 ap = argparse.ArgumentParser(); ap.add_argument("--out", default=None); ap.add_argument("--steps", type=int, default=20)
 args = ap.parse_args()
 peak = json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(
-    os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")) else 6650.0
+    os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")) else 3350.0
 flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev)
 
 

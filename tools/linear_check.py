@@ -1,4 +1,4 @@
-"""On-GPU check of pna_linear_fwd (3xTF32 tcgen05) against float64 and timing against cuBLAS fp32."""
+"""On-GPU check of pna_linear_fwd (3xTF32 wgmma) against float64 and timing against cuBLAS fp32."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
