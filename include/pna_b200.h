@@ -275,6 +275,16 @@ int pna_gather_rows(const void* src, int64_t ld_src, const int32_t* idx, int64_t
 int pna_halo_pull(const void* const* peer_rows, int64_t ld_rows, const int32_t* enc, int32_t peer_shift, int64_t n_idx, void* dst,
                   int64_t ld_dst, int32_t n_feat, int32_t dtype, pna_stream_t stream);
 
+/* The transpose of pna_halo_pull, for the backward: return the gradients of halo copies to the rows' owner.
+ * peer_rows: DEVICE array of n_ranks pointers, each to the start of that rank's fp32 halo-gradient rows (row pitch ld_rows
+ * elements on every rank), so the row index of a slot is a position in that rank's halo.  For i in [0, n_rows):
+ *     grad[rows[i], :] += sum over s in [rowptr[i], rowptr[i+1]) of  peer_rows[enc[s] >> enc_shift][enc[s] & mask, :]
+ * summed in slot order in fp32, one rounding per add, starting from the current grad row (pitch ld_grad).  rows must not
+ * repeat: each row is owned by one warp and there are no atomics, so with slots in a fixed order (ascending peer rank, as
+ * pna_b200/dist.py plans them) the result is bit-reproducible.  enc_shift in 1..30; n_rows == 0 launches nothing. */
+int pna_halo_grad_pull(const void* const* peer_rows, int64_t ld_rows, const int32_t* rows, const int32_t* rowptr, const int32_t* enc,
+                       int32_t enc_shift, int64_t n_rows, float* grad, int64_t ld_grad, int32_t n_feat, pna_stream_t stream);
+
 /* Device-side barrier between the ranks of one box, enqueued on `stream`: peer_flags is a DEVICE array of n_ranks pointers to
  * each rank's uint64 flags[n_ranks] (zero-initialised once, mapped into every process like the feature rows).  Rank r
  * stores `epoch` into flags[r] of every peer and waits until its own flags all reach `epoch`; epochs must increase by

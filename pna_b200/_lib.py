@@ -39,7 +39,7 @@ FLAG_ZERO_ISOLATED, FLAG_SKIP_LIGHT, FLAG_SKIP_HUBS, FLAG_RELU_VAR, FLAG_GATHER_
 # every symbol the header declares (checked by tests/test_abi.py)
 EXPORTED_SYMBOLS = ("pna_csr_workspace_bytes", "pna_csr_build", "pna_csr_light_view", "pna_csr_light_view_workspace_bytes", "pna_aggregate_fwd", "pna_aggregate_bwd",
                     "pna_aggregate_bwd_coef", "pna_aggregate_bwd_combine",
-                    "pna_gather_rows", "pna_halo_pull", "pna_peer_barrier", "pna_linear_fwd", "pna_linear_scaled_fwd", "pna_row_scales", "pna_linear_workspace_bytes", "pna_query", "pna_last_error")
+                    "pna_gather_rows", "pna_halo_pull", "pna_halo_grad_pull", "pna_peer_barrier", "pna_linear_fwd", "pna_linear_scaled_fwd", "pna_row_scales", "pna_linear_workspace_bytes", "pna_query", "pna_last_error")
 
 
 class PnaError(RuntimeError):
@@ -171,6 +171,9 @@ def lib() -> C.CDLL:
         L.pna_halo_pull.restype = C.c_int
         L.pna_halo_pull.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_int32,
                                     C.c_int32, C.c_void_p]
+        L.pna_halo_grad_pull.restype = C.c_int
+        L.pna_halo_grad_pull.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p,
+                                         C.c_int64, C.c_int32, C.c_void_p]
         L.pna_peer_barrier.restype = C.c_int
         L.pna_peer_barrier.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]
         L.pna_linear_workspace_bytes.restype = C.c_int

@@ -9,7 +9,8 @@ Three ways to reach remote source rows, all behind ``pna_aggregate_fwd``:
   per graph, locally (the puller names the rows; no id exchange); per layer a device-side flag barrier
   (``pna_peer_barrier``) and ONE kernel of NVLink peer loads (``pna_halo_pull``) fill the halo tail of the rank's
   ``[local ; halo]`` buffer, and the aggregation gathers from local HBM only.  A remote row crosses NVLink once per layer
-  however often it is gathered -- what a power-law graph needs.
+  however often it is gathered -- what a power-law graph needs.  The only plane with a backward
+  (``trainable=True``): the owners pull the halo rows' gradients back the same way (``pna_halo_grad_pull``).
 * ``halo`` (``HaloAggregator``; the north star's wording, measured beside pull): the same rows through a pack kernel
   (``pna_gather_rows``) and ONE NCCL all-to-all-v (``torch.distributed.all_to_all_single``); rows whose sources are all
   local can be reduced while the all-to-all is in flight (masked light views).
@@ -30,7 +31,7 @@ import torch
 import torch.distributed as dist
 
 from . import _lib
-from .aggregate import aggregate_forward
+from .aggregate import aggregate_forward, pna_aggregate
 from .csr import LightView, build_csr
 
 
@@ -201,6 +202,130 @@ def build_pull_plan(src_global: torch.Tensor, dst_global: torch.Tensor, bounds: 
     return PullPlan(rank, world, lo, hi, n_local, n_halo, shift, src_ext, dst_global - lo, halo_ids, enc, int(remote.sum()))
 
 
+# ---- the pull plane's backward: return halo gradients to their owners -------------------------------------------------
+@dataclass
+class GradReturnPlan:
+    """The owner's side of the pull plane's backward: which of this rank's rows its peers hold as halo copies, and where.
+    A compact CSR over the rows that have at least one copy; the slots of a row are in ascending peer rank, so
+    ``pna_halo_grad_pull`` adds them in a fixed order."""
+    rank: int
+    world: int
+    shift: int                     # enc = peer << shift | position in that peer's halo
+    rows: torch.Tensor             # int32 [n_rows] local rows held by at least one peer, ascending
+    rowptr: torch.Tensor           # int32 [n_rows + 1]
+    enc: torch.Tensor              # int32 [rowptr[-1]]
+    peer_n_local: List[int]        # every rank's n_local: where its halo-gradient rows start in its [local ; halo] buffer
+
+    @property
+    def n_rows(self) -> int:
+        return int(self.rows.numel())
+
+
+def grad_return_shift(max_halo: int, world: int) -> int:
+    """Bits for a halo position: enough for the largest halo of any rank (not the partition size of peer_shift_for)."""
+    shift = max(1, (max(int(max_halo), 1) - 1).bit_length())
+    if shift > 30 or (world << shift) >= 2 ** 31:
+        raise ValueError(f"halo of {max_halo} rows on {world} ranks is too large for the 32-bit peer|position encoding")
+    return shift
+
+
+def grad_return_plan(rank: int, world: int, held: List[torch.Tensor], offsets: List[int], max_halo: int,
+                     peer_n_local: List[int], device=None) -> GradReturnPlan:
+    """Owner ``rank``'s reverse plan from per-peer lists (pure; no communication).
+
+    held[p]   : int64, this rank's rows (owner-local ids, ascending) that rank p holds in its halo;
+    offsets[p]: position of the first of them in p's halo (p's halo ids are sorted, hence grouped by owner, so this rank's
+                rows are one contiguous segment of it and row held[p][i] sits at offsets[p] + i);
+    max_halo  : the largest n_halo of any rank -- it sizes the position field of the encoding."""
+    shift = grad_return_shift(max_halo, world)
+    if device is None:
+        device = held[0].device if held else torch.device("cpu")
+    rows_l, enc_l = [], []
+    for p in range(world):
+        ids = held[p].to(device=device, dtype=torch.int64)
+        if ids.numel() == 0:
+            continue
+        if p == rank:
+            raise ValueError("grad_return_plan: a rank cannot hold its own rows in its halo")
+        pos = int(offsets[p]) + torch.arange(ids.numel(), dtype=torch.int64, device=device)
+        rows_l.append(ids)
+        enc_l.append((p << shift) | pos)
+    if not rows_l:
+        empty = torch.zeros(0, dtype=torch.int32, device=device)
+        return GradReturnPlan(rank, world, shift, empty, torch.zeros(1, dtype=torch.int32, device=device), empty.clone(),
+                              list(map(int, peer_n_local)))
+    rows, enc = torch.cat(rows_l), torch.cat(enc_l)
+    order = torch.sort(rows, stable=True).indices          # peers were appended in rank order: stable keeps it per row
+    rows, enc = rows[order], enc[order]
+    uniq, counts = torch.unique_consecutive(rows, return_counts=True)
+    rowptr = torch.zeros(uniq.numel() + 1, dtype=torch.int64, device=device)
+    rowptr[1:] = torch.cumsum(counts, 0)
+    return GradReturnPlan(rank, world, shift, uniq.to(torch.int32), rowptr.to(torch.int32), enc.to(torch.int32),
+                          list(map(int, peer_n_local)))
+
+
+def _halo_segments(plan: PullPlan):
+    """(owner-local ids grouped by owner, rows per owner, offset of each owner's segment) of a puller's halo."""
+    own = (plan.enc >> plan.shift).to(torch.int64)
+    want = (plan.enc & ((1 << plan.shift) - 1)).to(torch.int64)
+    counts = torch.bincount(own, minlength=plan.world) if plan.n_halo else torch.zeros(plan.world, dtype=torch.int64,
+                                                                                          device=plan.enc.device)
+    offsets = torch.cumsum(counts, 0) - counts
+    return want, counts, offsets
+
+
+def grad_return_plans(plans: List[PullPlan]) -> List[GradReturnPlan]:
+    """Every rank's reverse plan from every rank's PullPlan, in one process (what build_grad_return_plan computes with
+    collectives)."""
+    world = len(plans)
+    max_halo = max(p.n_halo for p in plans)
+    n_local = [p.n_local for p in plans]
+    segs = [_halo_segments(p) for p in plans]
+    out = []
+    for r in range(world):
+        held, offs = [], []
+        for p in range(world):
+            want, counts, offsets = segs[p]
+            o, c = int(offsets[r]), int(counts[r])
+            held.append(want[o:o + c])
+            offs.append(o)
+        out.append(grad_return_plan(r, world, held, offs, max_halo, n_local, device=plans[r].enc.device))
+    return out
+
+
+def build_grad_return_plan(plan: PullPlan, group=None) -> GradReturnPlan:
+    """This rank's reverse plan, once per graph, with two collectives: an all-to-all of (row count, segment offset,
+    n_local, n_halo) per rank pair, then an all-to-all of the owner-local row ids (``build_halo_plan``'s pattern)."""
+    dev = plan.enc.device
+    world = plan.world
+    want, counts, offsets = _halo_segments(plan)
+    meta = torch.stack([counts, offsets, torch.full_like(counts, plan.n_local), torch.full_like(counts, plan.n_halo)], 1)
+    meta_in = torch.empty_like(meta)
+    dist.all_to_all_single(meta_in, meta.contiguous(), group=group)
+    recv_counts = meta_in[:, 0].tolist()
+    ids = torch.empty(sum(recv_counts), dtype=torch.int64, device=dev)
+    dist.all_to_all_single(ids, want, output_split_sizes=recv_counts, input_split_sizes=counts.tolist(), group=group)
+    held = list(torch.split(ids, recv_counts))
+    return grad_return_plan(plan.rank, world, held, meta_in[:, 1].tolist(), int(meta_in[:, 3].max()), meta_in[:, 2].tolist(),
+                            device=dev)
+
+
+class _HaloExchange(torch.autograd.Function):
+    """x [n_local, F] -> a fresh [n_local + n_halo, F] copy of [x ; halo]; backward returns the halo rows' gradients to
+    their owners (``PullAggregator.stage_halo_grad`` + ``pull_halo_grad``)."""
+
+    @staticmethod
+    def forward(ctx, x, agg):
+        ctx.agg, ctx.x_dtype = agg, x.dtype
+        return agg.exchange_features(x)
+
+    @staticmethod
+    def backward(ctx, grad_ext):
+        agg = ctx.agg
+        agg.stage_halo_grad(grad_ext)
+        return agg.pull_halo_grad(grad_ext).to(ctx.x_dtype), None
+
+
 class PullAggregator:
     """[local ; halo] source buffer whose halo tail is filled by ONE kernel of peer loads (``pna_halo_pull``): the
     all-to-all of the north star without a collective -- no id exchange when the graph is planned, no pack kernel, no
@@ -211,9 +336,21 @@ class PullAggregator:
     buffer.  The feature buffer is DOUBLE-BUFFERED (``flip()`` between layers / steps): a rank may already be writing
     layer l+1's rows while slower peers still pull layer l's, and the barrier of layer l+1 separates layer l's pulls
     from the writes of layer l+2 into the same buffer.
+
+    Training (``trainable=True``; opt-in, a forward-only aggregator allocates and communicates nothing more):
+    ``pna_aggregate(x, ...)`` is differentiable in ``x``.  Forward: ``x`` -> ``x_local``, barrier, pull, and a copy of
+    ``[x ; halo]`` that the next layers' reuse of the double buffers cannot overwrite (the backward reads it: n_local +
+    n_halo rows per layer), then ``flip()``.  Backward: the gradient of the halo rows goes into this rank's fp32 gradient
+    buffer (``stage_halo_grad``), then a barrier, then every owner pulls the gradients its peers hold for copies of its
+    rows and adds them into its own (``pull_halo_grad``, ``pna_halo_grad_pull``).  The slots of a row are added in
+    ascending peer rank, without atomics: the gradient return is bit-reproducible.  The gradient buffers alternate like
+    the feature buffers, by the same argument: backward exchange j+2 rewrites the buffer that peers pulled from in
+    exchange j only after this rank has passed barrier j+1, which no peer enters before its pull of exchange j is done.
+    Parameter gradients are this rank's partial sums; summing them across ranks (``all_reduce``) is the caller's job.
     """
 
-    def __init__(self, plan: PullPlan, n_feat: int, dtype=torch.float32, group=None, buffers: int = 2, _alloc=None):
+    def __init__(self, plan: PullPlan, n_feat: int, dtype=torch.float32, group=None, buffers: int = 2, _alloc=None,
+                 trainable: bool = False, grad_plan: Optional[GradReturnPlan] = None, _barrier=None):
         dev = plan.src_ext.device
         self.plan, self.group, self.n_feat, self.dtype = plan, group, n_feat, dtype
         self.csr = build_csr(plan.src_ext, plan.dst_local, plan.n_local, n_src=plan.n_local + max(plan.n_halo, 0))
@@ -233,8 +370,25 @@ class PullAggregator:
         self._keep.append(keep)
         self._status = torch.zeros(1, dtype=torch.int32, device=dev)
         self._epoch, self._cur = 0, 0
-        self.use_barrier = plan.world > 1 and _alloc is None
-        if self.use_barrier:   # flags are zero everywhere before the first flag store can arrive
+        # gradient return (trainable only): fp32 buffers whose halo tails the owners pull from, like the feature buffers
+        self.trainable, self.grad_plan = trainable, None
+        self._gbufs, self._gtables, self._gcur = [], [], 0
+        if trainable:
+            if grad_plan is None:
+                grad_plan = build_grad_return_plan(plan, group) if plan.world > 1 else grad_return_plan(
+                    plan.rank, 1, [torch.zeros(0, dtype=torch.int64, device=dev)], [0], plan.n_halo, [plan.n_local], device=dev)
+            if grad_plan.rank != plan.rank or grad_plan.world != plan.world:
+                raise ValueError("grad_plan belongs to another rank or world")
+            self.grad_plan = grad_plan
+            for _ in range(buffers):
+                t, ptrs, keep = alloc((int(rows), n_feat), torch.float32)
+                tails = [int(ptrs[p]) + grad_plan.peer_n_local[p] * n_feat * 4 for p in range(len(ptrs))]
+                self._gbufs.append(t)
+                self._gtables.append(torch.tensor(tails, dtype=torch.int64, device=dev))
+                self._keep.append(keep)
+        self._barrier_hook = _barrier      # host-side stand-in for the device barrier (several ranks in one process)
+        self.use_barrier = (plan.world > 1 and _alloc is None) or _barrier is not None
+        if self.use_barrier and _barrier is None:   # flags are zero everywhere before the first flag store can arrive
             torch.cuda.synchronize(dev)
             dist.barrier(group=group, device_ids=[dev.index])
 
@@ -251,6 +405,9 @@ class PullAggregator:
         self._cur = (self._cur + 1) % len(self._bufs)
 
     def barrier(self) -> None:
+        if self._barrier_hook is not None:
+            self._barrier_hook()
+            return
         self._epoch += 1
         dev = self._flags.device
         with torch.cuda.device(dev):
@@ -274,6 +431,63 @@ class PullAggregator:
     def aggregate(self, aggregators, scalers, avg_deg, out: Optional[torch.Tensor] = None, **kw) -> torch.Tensor:
         self.exchange()
         return aggregate_forward(self.x_ext, self.csr, aggregators, scalers, avg_deg, out=out, **kw)
+
+    # ---- differentiable path (trainable=True) ----
+    def exchange_features(self, x: torch.Tensor) -> torch.Tensor:
+        """Forward half of the differentiable exchange, without autograd: ``x`` -> ``x_local``, barrier, pull; returns a
+        fresh ``[n_local + n_halo, F]`` copy of ``[x ; halo]`` and flips to the other feature buffer."""
+        p = self.plan
+        if tuple(x.shape) != (p.n_local, self.n_feat) or x.dtype != self.dtype:
+            raise ValueError(f"x must be [{p.n_local}, {self.n_feat}] {self.dtype}, got {tuple(x.shape)} {x.dtype}")
+        self.x_local.copy_(x)
+        self.exchange()
+        out = self.x_ext.clone()
+        self.flip()
+        return out
+
+    def stage_halo_grad(self, grad_ext: torch.Tensor) -> None:
+        """Backward, first half: this rank's gradient for its halo rows -> the halo tail of its current fp32 gradient
+        buffer, where the rows' owners pull it from."""
+        p = self.plan
+        if not self.trainable:
+            raise RuntimeError("the gradient return needs PullAggregator(..., trainable=True)")
+        if p.n_halo:
+            self._gbufs[self._gcur][p.n_local:p.n_local + p.n_halo].copy_(grad_ext[p.n_local:p.n_local + p.n_halo])
+
+    def pull_halo_grad(self, grad_ext: torch.Tensor) -> torch.Tensor:
+        """Backward, second half: barrier, then a fp32 copy of ``grad_ext[:n_local]`` plus the gradients every peer staged
+        for copies of this rank's rows (``pna_halo_grad_pull``); flips to the other gradient buffer."""
+        p, gp = self.plan, self.grad_plan
+        if not self.trainable:
+            raise RuntimeError("the gradient return needs PullAggregator(..., trainable=True)")
+        if self.use_barrier:
+            self.barrier()
+        dev = self._gbufs[self._gcur].device
+        g = torch.empty((p.n_local, self.n_feat), dtype=torch.float32, device=dev)
+        g.copy_(grad_ext[:p.n_local])
+        if gp.n_rows:
+            with torch.cuda.device(dev):
+                _lib.check(_lib.lib().pna_halo_grad_pull(self._gtables[self._gcur].data_ptr(), self.n_feat, gp.rows.data_ptr(),
+                                                         gp.rowptr.data_ptr(), gp.enc.data_ptr(), gp.shift, gp.n_rows, g.data_ptr(),
+                                                         self.n_feat, self.n_feat, torch.cuda.current_stream(dev).cuda_stream))
+        self._gcur = (self._gcur + 1) % len(self._gbufs)
+        return g
+
+    def pna_aggregate(self, x: torch.Tensor, aggregators, scalers, avg_deg, *, towers: int = 1,
+                      row_bias: Optional[torch.Tensor] = None, self_feat: Optional[torch.Tensor] = None,
+                      self_divided: bool = True, zero_isolated: bool = False, relu_var: bool = False,
+                      scaler_degree: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Differentiable aggregation of this rank's rows (``pna_b200.pna_aggregate`` on ``[x ; halo]``): x is the rank's
+        ``[n_local, F]`` features, ``row_bias`` / ``self_feat`` are per destination and stay local; returns the rank's
+        ``[n_local, width]`` output.  Every rank must make the same sequence of calls (each one holds a barrier in the
+        forward and, if a gradient flows, one in the backward).  Gradients of parameters that produced ``x`` are
+        this rank's partial sums: all-reduce them across ranks before the optimizer step."""
+        if x.requires_grad and torch.is_grad_enabled() and not self.trainable:
+            raise RuntimeError("a gradient through the halo exchange needs PullAggregator(..., trainable=True)")
+        x_ext = _HaloExchange.apply(x, self)
+        return pna_aggregate(x_ext, self.csr, aggregators, scalers, avg_deg, towers=towers, row_bias=row_bias,
+                             self_feat=self_feat, self_divided=self_divided, zero_isolated=zero_isolated, relu_var=relu_var,
+                             scaler_degree=scaler_degree)
 
     def check(self) -> None:
         """Host-side check (synchronises): did every barrier see all peers arrive?"""

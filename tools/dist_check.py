@@ -1,4 +1,5 @@
-"""torchrun --nproc-per-node N tools/dist_check.py : multi-GPU parity of the peer and halo paths against the oracle."""
+"""torchrun --nproc-per-node N tools/dist_check.py : multi-GPU parity of the peer, halo and pull paths against the oracle,
+and of the pull path's backward (the gradient returned to every rank's rows) against the oracle's autograd."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch, torch.distributed as dist
@@ -41,6 +42,22 @@ for (n, e, f, hubdeg) in [(4000, 40000, 128, 3000), (3000, 20000, 64, 0), (5000,
         ha = pd.HaloAggregator(plan, f, overlap=ov)
         ha.x_local.copy_(x[lo:hi].to(dev))
         check(ha.aggregate(A4, S3, avg), f"halo overlap={ov} n_halo={plan.n_halo} interior={int(plan.interior.sum())}")
+    # pull path, forward and backward: the gradient every rank gets back for its rows against the oracle's autograd
+    pplan = pd.build_pull_plan(src[mine].to(dev), dst[mine].to(dev), bounds, rank, world)
+    pull = pd.PullAggregator(pplan, f, trainable=True)
+    w = torch.randn(n, 12 * f, generator=torch.Generator().manual_seed(f))
+    xr = x.clone().requires_grad_(True)
+    (O.simple_propagate(xr, torch.stack([src, dst]), A4, S3, avg) * w).sum().backward()
+    xm = x[lo:hi].to(dev).requires_grad_(True)
+    out = pull.pna_aggregate(xm, A4, S3, avg)
+    (out * w[lo:hi].to(dev)).sum().backward()
+    pull.check()
+    check(out.detach(), "pull")
+    gw, gg = xr.grad[lo:hi], xm.grad.cpu()
+    good = torch.allclose(gg, gw, rtol=1e-3, atol=5e-4)
+    ok &= good
+    print(f"rank {rank} n={n} f={f} pull backward: max err {(gg - gw).abs().max().item():.2e} "
+          f"return rows={pull.grad_plan.n_rows} {'ok' if good else 'MISMATCH'}", flush=True)
     torch.cuda.synchronize(); dist.barrier(device_ids=[local])
 t = torch.tensor([1 if ok else 0], device=dev); dist.all_reduce(t, op=dist.ReduceOp.MIN)
 if rank == 0: print("DIST ALL OK" if int(t) else "DIST FAILED")
