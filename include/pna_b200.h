@@ -261,6 +261,23 @@ int pna_aggregate_bwd_combine(const float* coef_sums, int64_t ld_sums, int32_t c
                               int64_t ld_gathered, int32_t dtype, float* grad_gathered, int64_t ld_grad_gathered, int64_t n_src,
                               int32_t n_feat, pna_stream_t stream);
 
+/* The same gradient with no floating-point atomics: a fixed function of the inputs and the graph (bit-reproducible).
+ * Per call one feature slab [f_begin, f_begin + f_count): f_begin a multiple of 4 (PNA_F32) / 8 (PNA_BF16), f_count too
+ * unless the slab ends at n_feat; otherwise PNA_ERR_BAD_ARG.  Two steps per slab:
+ *  1. pna_aggregate_bwd_slots: STORES the gradient of every message into grad_slots [E, f_count] fp32 (row = CSR slot,
+ *     column = feature - f_begin; ld_grad_slots >= f_count, 16-byte aligned rows get vector stores) -- the value the atomic
+ *     path adds into grad_gathered[col[slot]], bit for bit -- and writes columns [f_begin, f_begin + f_count) of
+ *     grad_row_bias (nullable, [n_rows, n_feat] fp32, addressed like pna_aggregate_bwd's), split rows as the chunks' slot-order
+ *     sums added in chunk order.  With desc->col == NULL (messages in CSR order) grad_slots IS the gradient of the messages.
+ *     desc->hub_partials as for pna_aggregate_bwd.  Peer-memory descriptors: PNA_ERR_UNSUPPORTED.
+ *  2. (desc->col != NULL) the caller sums grad_slots over the out-edges of every source row: pna_aggregate_fwd on the
+ *     slot-transposed CSR (pna_csr_build with src = slot id 0..E-1, dst = col, n_nodes = n_src: rows are source rows, slots
+ *     are forward slot ids in ascending order) with gathered = grad_slots, one aggregator PNA_AGGR_SUM, one scaler
+ *     PNA_SCALE_IDENTITY, out = the grad_gathered column slab.  The forward sums every row in a fixed order. */
+int pna_aggregate_bwd_slots(const pna_agg_t* desc, const void* grad_out, int64_t ld_grad_out, int32_t f_begin, int32_t f_count,
+                            float* grad_slots, int64_t ld_grad_slots, float* grad_row_bias, int64_t ld_grad_row_bias,
+                            pna_stream_t stream);
+
 /* ---- halo rows for the destination-partitioned multi-GPU path (north_star: "single NCCL all-to-all for halo
  * source features per layer"): dst[i, :] = src[idx[i], :], n_feat elements per row.  Used to pack the send buffer. */
 int pna_gather_rows(const void* src, int64_t ld_src, const int32_t* idx, int64_t n_idx, void* dst, int64_t ld_dst,

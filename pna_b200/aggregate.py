@@ -202,7 +202,11 @@ def aggregate_backward(grad_out: torch.Tensor, gathered: torch.Tensor, csr: CSRG
     grad_out = _rows2d(grad_out.to(gathered.dtype), "grad_out")
     if row_bias is not None:
         row_bias = _rows2d(row_bias.to(gathered.dtype), "row_bias")
-    gg = torch.zeros((gathered.size(0), F), dtype=torch.float32, device=dev)
+    deterministic = backward_mode() == "deterministic"
+    if deterministic and csr.n_edges:     # every element is written (per-slot stores, or the forward's sums per source row)
+        gg = torch.empty((gathered.size(0), F), dtype=torch.float32, device=dev)
+    else:
+        gg = torch.zeros((gathered.size(0), F), dtype=torch.float32, device=dev)
     gb = torch.empty((N, F), dtype=torch.float32, device=dev) if need_bias_grad else None
     d = _lib.AggStruct(
         gathered=_ptr(gathered), ld_gathered=gathered.stride(0) if gathered.size(0) > 1 else F,
@@ -223,6 +227,9 @@ def aggregate_backward(grad_out: torch.Tensor, gathered: torch.Tensor, csr: CSRG
         scratch = torch.empty(((csr.n_chunks + csr.n_hubs) * 6, F), dtype=torch.float32, device=dev)
         d.hub_partials = scratch.data_ptr()
     ld_go = grad_out.stride(0) if N > 1 else grad_out.size(1)
+    if deterministic:
+        _backward_deterministic(d, grad_out, ld_go, gathered, csr, gg, gb, messages_in_csr_order)
+        return gg, gb
     if messages_in_csr_order or csr.n_edges == 0 or csr.sources_unique or backward_mode() == "atomic" \
             or 2 * _round_up(F, 4) > _lib.query(_lib.QUERY_MAX_FEATURES):
         with torch.cuda.device(dev):
@@ -248,12 +255,58 @@ def _round_up(n: int, m: int) -> int:
     return (n + m - 1) // m * m
 
 
+# Bound on the fp32 per-slot gradients [E, slab] of the deterministic backward: wider rows are done in feature slabs.
+DETERMINISTIC_SCRATCH_BYTES = 1 << 30
+
+
+def deterministic_slab_width(n_edges: int, n_feat: int, align: int) -> int:
+    """Feature columns per slab of the deterministic backward: all of them if ``E * F * 4`` bytes fit
+    DETERMINISTIC_SCRATCH_BYTES, else the widest multiple of ``align`` (16 bytes of the element type) that does; never more
+    than the forward kernel takes (PNA_QUERY_MAX_FEATURES), which sums the slab over the reversed edges."""
+    max_f = _lib.query(_lib.QUERY_MAX_FEATURES) // align * align
+    if n_edges * n_feat * 4 <= DETERMINISTIC_SCRATCH_BYTES and n_feat <= max_f:
+        return n_feat
+    w = DETERMINISTIC_SCRATCH_BYTES // (4 * max(n_edges, 1)) // align * align
+    return max(align, min(w, max_f))
+
+
+def _backward_deterministic(d, grad_out, ld_go, gathered, csr: CSRGraph, gg, gb, messages_in_csr_order: bool) -> None:
+    """No floating-point atomics: per feature slab, (1) ``pna_aggregate_bwd_slots`` stores the gradient of every message in
+    CSR slot order, (2) the forward kernel sums those rows over the slot-transposed CSR (ascending slot ids per source row)
+    into the ``gg`` column slab.  Messages in CSR order need step 1 only: its output is their gradient."""
+    dev = gathered.device
+    F, E = gg.size(1), csr.n_edges
+    L = _lib.lib()
+    stream = torch.cuda.current_stream(dev).cuda_stream
+    if messages_in_csr_order:
+        gs = gg if E else torch.empty((1, F), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(L.pna_aggregate_bwd_slots(C.byref(d), grad_out.data_ptr(), ld_go, 0, F, gs.data_ptr(), F, _ptr(gb), F, stream))
+        return
+    w = deterministic_slab_width(E, F, 16 // gathered.element_size())
+    buf = torch.empty(max(E, 1) * w, dtype=torch.float32, device=dev)
+    tcsr = csr.slot_transposed(gathered.size(0)) if E else None
+    for f0 in range(0, F, w):
+        fc = min(w, F - f0)
+        gs = buf[:max(E, 1) * fc].view(max(E, 1), fc)
+        with torch.cuda.device(dev):
+            _lib.check(L.pna_aggregate_bwd_slots(C.byref(d), grad_out.data_ptr(), ld_go, f0, fc, gs.data_ptr(), fc, _ptr(gb), F,
+                                                 stream))
+        if E:
+            aggregate_forward(gs, tcsr, ["sum"], ["identity"], {"log": 1.0, "lin": 1.0}, out=gg[:, f0:f0 + fc])
+
+
 def backward_mode() -> str:
     """Which backward runs for gathered rows: "atomic" (default) = ``pna_aggregate_bwd``, one call, a vector atomic per edge and
     feature chunk; ``PNA_B200_BWD=coef`` = per-destination coefficient rows (``pna_aggregate_bwd_coef``), their sums over the
     transposed graph through the forward kernels, ``pna_aggregate_bwd_combine`` -- atomics only for min / max.  The
     coefficient path avoids the atomics that contend on hot source rows (power-law graphs), but regrouping sum_i (c0_i + c1_i x_j) into sum_i c0_i + x_j sum_i c1_i cancels badly where many rows have var ~ 0
-    (2.6x the fp32 error of the per-edge evaluation on a power-law multigraph), so it stays opt-in."""
+    (2.6x the fp32 error of the per-edge evaluation on a power-law multigraph), so it stays opt-in.
+    Under ``torch.use_deterministic_algorithms(True)`` (``warn_only`` too) "deterministic", whatever PNA_B200_BWD says: per-slot
+    gradients (``pna_aggregate_bwd_slots``) summed over the reversed edges by the forward kernel, no floating-point atomics,
+    the same bits on every run."""
+    if torch.are_deterministic_algorithms_enabled():
+        return "deterministic"
     return "coef" if os.environ.get("PNA_B200_BWD", "atomic") == "coef" else "atomic"
 
 

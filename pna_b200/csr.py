@@ -115,6 +115,17 @@ class CSRGraph:
             self._partials[key] = t
         return t
 
+    def slot_transposed(self, n_src: int) -> "CSRGraph":
+        """CSR of the reversed edges whose slots are the forward CSR slot ids (rows = the ``n_src`` source rows, each row's slot
+        ids in ascending order): what the deterministic backward sums its per-slot gradients over (pna_aggregate_bwd_slots).
+        Built on first use, kept with the graph."""
+        key = ("S", int(n_src))
+        t = self._partials.get(key)
+        if t is None:
+            t = build_csr(torch.arange(self.n_edges, device=self.device), self.col.long(), int(n_src), n_src=self.n_edges)
+            self._partials[key] = t
+        return t
+
     def masked_view(self, row_mask: torch.Tensor) -> LightView:
         """Light view of the rows with ``row_mask != 0`` only (uint8/bool [N]); other rows are skipped by the kernel."""
         N, dev = self.n_nodes, self.device

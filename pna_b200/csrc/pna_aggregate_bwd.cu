@@ -18,6 +18,12 @@
 // scalar atomic per (row, feature) and writes grad_row_bias in closed form (deg * c0 + c1 * sum_m + gmin + gmax).  The two
 // sums over the out-edges are a 'sum' aggregation of those rows over the transposed graph (pna_aggregate_fwd, no atomics),
 // folded into grad_gathered by pna_aggregate_bwd_combine.
+//
+// pna_aggregate_bwd_slots (the deterministic backward): the same kernels compiled with SLOTS = true.  Pass C STORES grad_m of
+// every slot into grad_slots[slot] (one feature slab [f_begin, f_begin + f_count) per call) instead of adding it into
+// grad_gathered[col[slot]]; the caller sums those rows over the reversed edges with the forward kernel (fixed order).  Split
+// rows store each chunk's share of grad_row_bias in scratch and k_bwd_hub_bias adds the shares in chunk order.  No
+// floating-point atomics in any kernel of this variant.
 #include "pna_aggregate.cuh"
 #include <string.h>
 
@@ -31,7 +37,16 @@ struct BParams {
   int vec_atomics;                    // grad_gathered rows are 16-byte aligned
   float* coef; long long ldc;         // coefficient mode (pna_aggregate_bwd_coef): [n_rows, ldc] rows [c0' | c1], c1 at column coef_c1
   int coef_c1, coef_vec;
+  float* gs; long long ldgs;          // per-slot mode (pna_aggregate_bwd_slots): grad_slots [E, f1 - f0] fp32, written
+  int f0, f1;                         // feature slab [f0, f1) of the per-slot mode
+  int gs_vec;                         // grad_slots rows are 16-byte aligned
 };
+
+// Gradient of one message, grad_m = c0 + c1 * m + [slot == argmin] gmin + [slot == argmax] gmax, every operation rounded on
+// its own and added left to right.  The atomic and the per-slot kernels share it, so both see the same value of every slot.
+__device__ __forceinline__ float message_grad(float c0, float c1, float m, bool is_min, float gmin, bool is_max, float gmax) {
+  return __fadd_rn(__fadd_rn(__fadd_rn(c0, __fmul_rn(c1, m)), is_min ? gmin : 0.f), is_max ? gmax : 0.f);
+}
 
 template <int VEC>
 struct Stats {
@@ -152,6 +167,33 @@ __device__ __forceinline__ LaneCols lane_cols(const KParams& p, int gl, int fblo
   return c;
 }
 
+// columns of this lane in this block: all n_feat columns, or (per-slot mode) the slab [f0, f1)
+template <int VEC, int G, bool SLOTS>
+__device__ __forceinline__ LaneCols block_cols(const BParams& b, int gl) {
+  if constexpr (SLOTS) {
+    LaneCols c = lane_cols<VEC>(b.k, gl, b.f0 + (int)blockIdx.y * (G * VEC));
+    if (c.f >= b.f1) c.ok = false;
+    return c;
+  } else {
+    return lane_cols<VEC>(b.k, gl, blockIdx.y * (G * VEC));
+  }
+}
+
+// per-slot mode: grad_slots[slot, f - f0] = gm (plain stores)
+template <int VEC>
+__device__ __forceinline__ void store_slot(const BParams& b, int slot, int f, const float (&gm)[VEC]) {
+  float* dst = b.gs + (long long)slot * b.ldgs + (f - b.f0);
+  if constexpr (VEC % 4 == 0) {
+    if (b.gs_vec) {
+#pragma unroll
+      for (int i = 0; i < VEC; i += 4) *reinterpret_cast<float4*>(dst + i) = make_float4(gm[i], gm[i + 1], gm[i + 2], gm[i + 3]);
+      return;
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < VEC; ++i) dst[i] = gm[i];
+}
+
 // coefficient mode: what one destination row hands to its sources.  c0' = c0 + c1 * bias; min / max go to the source of the
 // one slot that attained them (st.amn / st.amx: absolute CSR slots, -1 = none); grad_row_bias in closed form.
 template <int VEC>
@@ -192,14 +234,14 @@ __device__ __forceinline__ void emit_row(const BParams& b, long long row, int de
 constexpr int kBwdThreads = 256;
 
 // ---- rows below the split threshold: one lane group per row --------------------------------------------------------
-template <typename T, int VEC, int G>
+template <typename T, int VEC, int G, bool SLOTS>
 __global__ void __launch_bounds__(kBwdThreads) k_bwd_rows(const BParams b) {
   const KParams& p = b.k;
   constexpr int RPW = 32 / G;
   const int lane = threadIdx.x & 31, gl = lane % G;
   const long long row = ((long long)blockIdx.x * (kBwdThreads / 32) + (threadIdx.x >> 5)) * RPW + lane / G;
   if (row >= p.n_rows) return;
-  const LaneCols lc = lane_cols<VEC>(p, gl, blockIdx.y * (G * VEC));
+  const LaneCols lc = block_cols<VEC, G, SLOTS>(b, gl);
   if (!lc.ok) return;
   const int beg = __ldg(p.rowptr + row), end = __ldg(p.rowptr + row + 1), deg = end - beg;
   if (deg >= p.split) return;
@@ -241,9 +283,11 @@ __global__ void __launch_bounds__(kBwdThreads) k_bwd_rows(const BParams b) {
   }
   Coef<VEC> c;
   coefficients<T, VEC>(b, row, deg, lc.ooff, st, c);
-  if (b.coef) {   // coefficient mode: no second pass over the slots
-    emit_row<VEC>(b, row, deg, lc, st, c, bias, has_bias);
-    return;
+  if constexpr (!SLOTS) {
+    if (b.coef) {   // coefficient mode: no second pass over the slots
+      emit_row<VEC>(b, row, deg, lc, st, c, bias, has_bias);
+      return;
+    }
   }
   float gbs[VEC];
 #pragma unroll
@@ -263,10 +307,11 @@ __global__ void __launch_bounds__(kBwdThreads) k_bwd_rows(const BParams b) {
 #pragma unroll
         for (int i = 0; i < VEC; ++i) {
           if (has_bias) m[i] = __fadd_rn(m[i], bias[i]);
-          gm[i] = c.c0[i] + c.c1[i] * m[i] + (e + u == st.amn[i] ? c.gmin[i] : 0.f) + (e + u == st.amx[i] ? c.gmax[i] : 0.f);
+          gm[i] = message_grad(c.c0[i], c.c1[i], m[i], e + u == st.amn[i], c.gmin[i], e + u == st.amx[i], c.gmax[i]);
           gbs[i] += gm[i];
         }
-        scatter_grad<VEC>(b, src[u], lc.f, gm, p.col != nullptr);
+        if constexpr (SLOTS) store_slot<VEC>(b, e + u, lc.f, gm);
+        else scatter_grad<VEC>(b, src[u], lc.f, gm, p.col != nullptr);
       }
     }
   }
@@ -282,14 +327,16 @@ __global__ void __launch_bounds__(kBwdThreads) k_bwd_rows(const BParams b) {
 //                      and turns the upstream gradient into (c0, c1, gmin, gmax, argmin, argmax) per feature;
 // (3) k_bwd_hub_scatter: one lane group per chunk evaluates grad_m per slot, scatters it, and adds its share of the
 //                      row_bias gradient.  Scratch (descriptor field hub_partials): 6*F floats per chunk + per split row.
-template <typename T, int VEC, int G>
+// Per-slot mode: (3) stores grad_m per slot and parks the chunk's row_bias share in the chunk's (consumed) sum partial;
+// (4) k_bwd_hub_bias: one lane group per split row adds those shares in chunk order.
+template <typename T, int VEC, int G, bool SLOTS>
 __global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_stats(const BParams b) {
   const KParams& p = b.k;
   constexpr int RPW = 32 / G;
   const int lane = threadIdx.x & 31, gl = lane % G;
   const long long c = ((long long)blockIdx.x * (kBwdThreads / 32) + (threadIdx.x >> 5)) * RPW + lane / G;
   if (c >= p.n_chunks) return;
-  const LaneCols lc = lane_cols<VEC>(p, gl, blockIdx.y * (G * VEC));
+  const LaneCols lc = block_cols<VEC, G, SLOTS>(b, gl);
   if (!lc.ok) return;
   const int h = __ldg(p.chunk_items + 2 * c), j = __ldg(p.chunk_items + 2 * c + 1);
   const long long row = __ldg(p.hub_info + 4 * h);
@@ -329,14 +376,14 @@ __global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_stats(const BParams b) 
   }
 }
 
-template <typename T, int VEC, int G>
+template <typename T, int VEC, int G, bool SLOTS>
 __global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_coef(const BParams b) {
   const KParams& p = b.k;
   constexpr int RPW = 32 / G;
   const int lane = threadIdx.x & 31, gl = lane % G;
   const long long h = ((long long)blockIdx.x * (kBwdThreads / 32) + (threadIdx.x >> 5)) * RPW + lane / G;
   if (h >= p.n_hubs) return;
-  const LaneCols lc = lane_cols<VEC>(p, gl, blockIdx.y * (G * VEC));
+  const LaneCols lc = block_cols<VEC, G, SLOTS>(b, gl);
   if (!lc.ok) return;
   const long long row = __ldg(p.hub_info + 4 * h);
   const int first = __ldg(p.hub_info + 4 * h + 1), nch = __ldg(p.hub_info + 4 * h + 2), deg = __ldg(p.hub_info + 4 * h + 3);
@@ -354,14 +401,16 @@ __global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_coef(const BParams b) {
   }
   Coef<VEC> c;
   coefficients<T, VEC>(b, row, deg, lc.ooff, st, c);
-  if (b.coef) {   // coefficient mode: the split row ends here, like every other row
-    const bool has_bias = p.bias != nullptr;
-    float bias[VEC];
+  if constexpr (!SLOTS) {
+    if (b.coef) {   // coefficient mode: the split row ends here, like every other row
+      const bool has_bias = p.bias != nullptr;
+      float bias[VEC];
 #pragma unroll
-    for (int i = 0; i < VEC; ++i) bias[i] = 0.f;
-    if (has_bias) Io<T, VEC>::load(static_cast<const T*>(p.bias) + row * p.ldb + lc.f, bias);
-    emit_row<VEC>(b, row, deg, lc, st, c, bias, has_bias);
-    return;
+      for (int i = 0; i < VEC; ++i) bias[i] = 0.f;
+      if (has_bias) Io<T, VEC>::load(static_cast<const T*>(p.bias) + row * p.ldb + lc.f, bias);
+      emit_row<VEC>(b, row, deg, lc, st, c, bias, has_bias);
+      return;
+    }
   }
   float* co = p.partials + (p.n_chunks + h) * 6ll * p.F + lc.f;
 #pragma unroll
@@ -369,20 +418,22 @@ __global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_coef(const BParams b) {
     co[0ll * p.F + i] = c.c0[i]; co[1ll * p.F + i] = c.c1[i]; co[2ll * p.F + i] = c.gmin[i]; co[3ll * p.F + i] = c.gmax[i];
     co[4ll * p.F + i] = __int_as_float(st.amn[i]); co[5ll * p.F + i] = __int_as_float(st.amx[i]);
   }
-  if (b.gb) {   // the chunks add their shares atomically in pass 3
+  if constexpr (!SLOTS) {
+    if (b.gb) {   // the chunks add their shares atomically in pass 3
 #pragma unroll
-    for (int i = 0; i < VEC; ++i) b.gb[row * b.ldgb + lc.f + i] = 0.f;
+      for (int i = 0; i < VEC; ++i) b.gb[row * b.ldgb + lc.f + i] = 0.f;
+    }
   }
 }
 
-template <typename T, int VEC, int G>
+template <typename T, int VEC, int G, bool SLOTS>
 __global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_scatter(const BParams b) {
   const KParams& p = b.k;
   constexpr int RPW = 32 / G;
   const int lane = threadIdx.x & 31, gl = lane % G;
   const long long c = ((long long)blockIdx.x * (kBwdThreads / 32) + (threadIdx.x >> 5)) * RPW + lane / G;
   if (c >= p.n_chunks) return;
-  const LaneCols lc = lane_cols<VEC>(p, gl, blockIdx.y * (G * VEC));
+  const LaneCols lc = block_cols<VEC, G, SLOTS>(b, gl);
   if (!lc.ok) return;
   const int h = __ldg(p.chunk_items + 2 * c), j = __ldg(p.chunk_items + 2 * c + 1);
   const long long row = __ldg(p.hub_info + 4 * h);
@@ -418,52 +469,88 @@ __global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_scatter(const BParams b
 #pragma unroll
         for (int i = 0; i < VEC; ++i) {
           if (has_bias) m[i] = __fadd_rn(m[i], bias[i]);
-          gm[i] = cf.c0[i] + cf.c1[i] * m[i] + (e + u == amn[i] ? cf.gmin[i] : 0.f) + (e + u == amx[i] ? cf.gmax[i] : 0.f);
+          gm[i] = message_grad(cf.c0[i], cf.c1[i], m[i], e + u == amn[i], cf.gmin[i], e + u == amx[i], cf.gmax[i]);
           gbs[i] += gm[i];
         }
-        scatter_grad<VEC>(b, src[u], lc.f, gm, p.col != nullptr);
+        if constexpr (SLOTS) store_slot<VEC>(b, e + u, lc.f, gm);
+        else scatter_grad<VEC>(b, src[u], lc.f, gm, p.col != nullptr);
       }
     }
   }
   if (b.gb) {
+    if constexpr (SLOTS) {   // this chunk's share, merged in chunk order by k_bwd_hub_bias (k_bwd_hub_coef has read the stats)
+      float* part = p.partials + c * 6ll * p.F + lc.f;
 #pragma unroll
-    for (int i = 0; i < VEC; ++i) atomicAdd(b.gb + row * b.ldgb + lc.f + i, gbs[i]);
+      for (int i = 0; i < VEC; ++i) part[i] = gbs[i];
+    } else {
+#pragma unroll
+      for (int i = 0; i < VEC; ++i) atomicAdd(b.gb + row * b.ldgb + lc.f + i, gbs[i]);
+    }
   }
 }
 
-template <typename T, int VEC, int G>
+// per-slot mode, split rows: grad_row_bias = the chunks' shares added in chunk order (each share in slot order)
+template <int VEC, int G>
+__global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_bias(const BParams b) {
+  const KParams& p = b.k;
+  constexpr int RPW = 32 / G;
+  const int lane = threadIdx.x & 31, gl = lane % G;
+  const long long h = ((long long)blockIdx.x * (kBwdThreads / 32) + (threadIdx.x >> 5)) * RPW + lane / G;
+  if (h >= p.n_hubs) return;
+  const LaneCols lc = block_cols<VEC, G, true>(b, gl);
+  if (!lc.ok) return;
+  const long long row = __ldg(p.hub_info + 4 * h);
+  const int first = __ldg(p.hub_info + 4 * h + 1), nch = __ldg(p.hub_info + 4 * h + 2);
+  float acc[VEC];
+#pragma unroll
+  for (int i = 0; i < VEC; ++i) acc[i] = 0.f;
+  for (int j = 0; j < nch; ++j) {
+    const float* part = p.partials + (long long)(first + j) * 6ll * p.F + lc.f;
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) acc[i] = __fadd_rn(acc[i], part[i]);
+  }
+#pragma unroll
+  for (int i = 0; i < VEC; ++i) b.gb[row * b.ldgb + lc.f + i] = acc[i];
+}
+
+template <typename T, int VEC, int G, bool SLOTS>
 static int launch_bwd(const BParams& b, cudaStream_t st) {
   const KParams& p = b.k;
   constexpr int RPW = 32 / G;
-  const unsigned gy = (unsigned)((p.F + G * VEC - 1) / (G * VEC));
+  const int width = SLOTS ? b.f1 - b.f0 : p.F;     // the per-slot mode covers one feature slab
+  const unsigned gy = (unsigned)((width + G * VEC - 1) / (G * VEC));
   const long long per_block = (kBwdThreads / 32) * RPW;
   const long long gx = (p.n_rows + per_block - 1) / per_block;
   PNA_REQUIRE(gx <= 0x7fffffffll, PNA_ERR_UNSUPPORTED, "pna_aggregate_bwd: too many rows");
-  k_bwd_rows<T, VEC, G><<<dim3((unsigned)gx, gy), kBwdThreads, 0, st>>>(b);
+  k_bwd_rows<T, VEC, G, SLOTS><<<dim3((unsigned)gx, gy), kBwdThreads, 0, st>>>(b);
   PNA_CUDA_TRY(cudaGetLastError());
   if (p.n_hubs > 0) {
     const long long gc = (p.n_chunks + per_block - 1) / per_block, gh = (p.n_hubs + per_block - 1) / per_block;
-    k_bwd_hub_stats<T, VEC, G><<<dim3((unsigned)gc, gy), kBwdThreads, 0, st>>>(b);
+    k_bwd_hub_stats<T, VEC, G, SLOTS><<<dim3((unsigned)gc, gy), kBwdThreads, 0, st>>>(b);
     PNA_CUDA_TRY(cudaGetLastError());
-    k_bwd_hub_coef<T, VEC, G><<<dim3((unsigned)gh, gy), kBwdThreads, 0, st>>>(b);
+    k_bwd_hub_coef<T, VEC, G, SLOTS><<<dim3((unsigned)gh, gy), kBwdThreads, 0, st>>>(b);
     PNA_CUDA_TRY(cudaGetLastError());
     if (!b.coef) {
-      k_bwd_hub_scatter<T, VEC, G><<<dim3((unsigned)gc, gy), kBwdThreads, 0, st>>>(b);
+      k_bwd_hub_scatter<T, VEC, G, SLOTS><<<dim3((unsigned)gc, gy), kBwdThreads, 0, st>>>(b);
+      PNA_CUDA_TRY(cudaGetLastError());
+    }
+    if (SLOTS && b.gb) {
+      k_bwd_hub_bias<VEC, G><<<dim3((unsigned)gh, gy), kBwdThreads, 0, st>>>(b);
       PNA_CUDA_TRY(cudaGetLastError());
     }
   }
   return PNA_OK;
 }
 
-template <typename T, int VEC>
+template <typename T, int VEC, bool SLOTS>
 static int launch_bwd_typed(const BParams& b, cudaStream_t st) {
-  const int chunks = b.k.F / VEC;
-  if (chunks <= 1) return launch_bwd<T, VEC, 1>(b, st);
-  if (chunks <= 2) return launch_bwd<T, VEC, 2>(b, st);
-  if (chunks <= 4) return launch_bwd<T, VEC, 4>(b, st);
-  if (chunks <= 8) return launch_bwd<T, VEC, 8>(b, st);
-  if (chunks <= 16) return launch_bwd<T, VEC, 16>(b, st);
-  return launch_bwd<T, VEC, 32>(b, st);     // wider rows: several feature blocks (gridDim.y)
+  const int chunks = (SLOTS ? b.f1 - b.f0 : b.k.F) / VEC;
+  if (chunks <= 1) return launch_bwd<T, VEC, 1, SLOTS>(b, st);
+  if (chunks <= 2) return launch_bwd<T, VEC, 2, SLOTS>(b, st);
+  if (chunks <= 4) return launch_bwd<T, VEC, 4, SLOTS>(b, st);
+  if (chunks <= 8) return launch_bwd<T, VEC, 8, SLOTS>(b, st);
+  if (chunks <= 16) return launch_bwd<T, VEC, 16, SLOTS>(b, st);
+  return launch_bwd<T, VEC, 32, SLOTS>(b, st);     // wider rows: several feature blocks (gridDim.y)
 }
 
 static bool al16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15u) == 0; }
@@ -489,17 +576,27 @@ __global__ void __launch_bounds__(256) k_bwd_combine(const float* __restrict__ s
 
 using namespace pna;
 
+// grad_slots != NULL: the per-slot mode (pna_aggregate_bwd_slots) over the feature slab [f_begin, f_begin + f_count)
 static int bwd_entry(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_out, float* grad_gathered, int64_t ld_grad_gathered,
                      float* grad_row_bias, int64_t ld_grad_row_bias, float* coef, int64_t ld_coef, int32_t coef_c1,
-                     pna_stream_t stream) {
+                     pna_stream_t stream, float* grad_slots = nullptr, int64_t ld_grad_slots = 0, int32_t f_begin = 0,
+                     int32_t f_count = 0) {
   PNA_REQUIRE(d != nullptr, PNA_ERR_BAD_ARG, "pna_aggregate_bwd: null descriptor");
   PNA_REQUIRE(d->n_rows >= 0 && d->n_feat > 0 && d->n_towers > 0 && d->n_feat % d->n_towers == 0, PNA_ERR_BAD_ARG,
               "pna_aggregate_bwd: bad sizes");
   PNA_REQUIRE(d->n_aggr >= 1 && d->n_aggr <= PNA_MAX_AGGR && d->n_scalers >= 1 && d->n_scalers <= PNA_MAX_SCALERS, PNA_ERR_BAD_ARG,
               "pna_aggregate_bwd: n_aggr / n_scalers out of range");
   PNA_REQUIRE(d->dtype == PNA_F32 || d->dtype == PNA_BF16, PNA_ERR_UNSUPPORTED, "pna_aggregate_bwd: dtype %d", d->dtype);
+  const bool slots = grad_slots != nullptr;
+  if (slots) {   // slabs start and (but for the last) end on a 16-byte boundary of the element type
+    const int al = d->dtype == PNA_F32 ? 4 : 8;
+    PNA_REQUIRE(f_begin >= 0 && f_count >= 1 && (long long)f_begin + f_count <= d->n_feat && f_begin % al == 0 &&
+                    (f_count % al == 0 || f_begin + f_count == d->n_feat),
+                PNA_ERR_BAD_ARG, "pna_aggregate_bwd_slots: bad feature slab [%d, +%d) of %d features", f_begin, f_count, d->n_feat);
+    PNA_REQUIRE(ld_grad_slots >= f_count, PNA_ERR_BAD_ARG, "pna_aggregate_bwd_slots: ld_grad_slots < f_count");
+  }
   if (d->n_rows == 0) return PNA_OK;
-  PNA_REQUIRE(d->gathered && d->rowptr && grad_out && grad_gathered, PNA_ERR_BAD_ARG, "pna_aggregate_bwd: null pointer");
+  PNA_REQUIRE(d->gathered && d->rowptr && grad_out && (slots || grad_gathered), PNA_ERR_BAD_ARG, "pna_aggregate_bwd: null pointer");
   PNA_REQUIRE(d->peer_gathered == nullptr, PNA_ERR_UNSUPPORTED, "pna_aggregate_bwd: peer-memory graphs are forward-only");
   PNA_REQUIRE(d->ld_gathered < 0x3fffffffll, PNA_ERR_UNSUPPORTED, "pna_aggregate_bwd: row pitch too large");
   PNA_REQUIRE(d->split_threshold >= 2, PNA_ERR_BAD_ARG, "pna_aggregate_bwd: bad split threshold");
@@ -535,19 +632,36 @@ static int bwd_entry(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_o
     b.coef = coef; b.ldc = ld_coef; b.coef_c1 = coef_c1;
     b.coef_vec = al16(coef) && (ld_coef % 4 == 0) && (coef_c1 % 4 == 0);
   }
+  if (slots) {
+    b.gs = grad_slots; b.ldgs = ld_grad_slots;
+    b.f0 = f_begin; b.f1 = f_begin + f_count;
+    b.gs_vec = al16(grad_slots) && (ld_grad_slots % 4 == 0);
+  }
 
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int esz = d->dtype == PNA_F32 ? 4 : 2;
   const int vec = 16 / esz;
   bool vec_ok = (p.Ft % vec == 0) && al16(p.x) && al16(grad_out) && (p.ldx % vec == 0) && (b.ldgo % vec == 0);
   if (p.bias) vec_ok = vec_ok && al16(p.bias) && (p.ldb % vec == 0);
-  if (d->dtype == PNA_F32) return vec_ok ? launch_bwd_typed<float, 4>(b, st) : launch_bwd_typed<float, 1>(b, st);
-  return vec_ok ? launch_bwd_typed<__nv_bfloat16, 8>(b, st) : launch_bwd_typed<__nv_bfloat16, 1>(b, st);
+  if (slots) {
+    if (d->dtype == PNA_F32) return vec_ok ? launch_bwd_typed<float, 4, true>(b, st) : launch_bwd_typed<float, 1, true>(b, st);
+    return vec_ok ? launch_bwd_typed<__nv_bfloat16, 8, true>(b, st) : launch_bwd_typed<__nv_bfloat16, 1, true>(b, st);
+  }
+  if (d->dtype == PNA_F32) return vec_ok ? launch_bwd_typed<float, 4, false>(b, st) : launch_bwd_typed<float, 1, false>(b, st);
+  return vec_ok ? launch_bwd_typed<__nv_bfloat16, 8, false>(b, st) : launch_bwd_typed<__nv_bfloat16, 1, false>(b, st);
 }
 
 extern "C" int pna_aggregate_bwd(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_out, float* grad_gathered,
                                  int64_t ld_grad_gathered, float* grad_row_bias, int64_t ld_grad_row_bias, pna_stream_t stream) {
   return bwd_entry(d, grad_out, ld_grad_out, grad_gathered, ld_grad_gathered, grad_row_bias, ld_grad_row_bias, nullptr, 0, 0, stream);
+}
+
+extern "C" int pna_aggregate_bwd_slots(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_out, int32_t f_begin, int32_t f_count,
+                                       float* grad_slots, int64_t ld_grad_slots, float* grad_row_bias, int64_t ld_grad_row_bias,
+                                       pna_stream_t stream) {
+  PNA_REQUIRE(grad_slots != nullptr, PNA_ERR_BAD_ARG, "pna_aggregate_bwd_slots: null grad_slots");
+  return bwd_entry(d, grad_out, ld_grad_out, nullptr, 0, grad_row_bias, ld_grad_row_bias, nullptr, 0, 0, stream, grad_slots,
+                   ld_grad_slots, f_begin, f_count);
 }
 
 extern "C" int pna_aggregate_bwd_coef(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_out, float* coef, int64_t ld_coef,
