@@ -9,11 +9,13 @@ Three ways to reach remote source rows, all behind ``pna_aggregate_fwd``:
   per graph, locally (the puller names the rows; no id exchange); per layer a device-side flag barrier
   (``pna_peer_barrier``) and ONE kernel of NVLink peer loads (``pna_halo_pull``) fill the halo tail of the rank's
   ``[local ; halo]`` buffer, and the aggregation gathers from local HBM only.  A remote row crosses NVLink once per layer
-  however often it is gathered -- what a power-law graph needs.  The only plane with a backward
-  (``trainable=True``): the owners pull the halo rows' gradients back the same way (``pna_halo_grad_pull``).
+  however often it is gathered -- what a power-law graph needs.  Trainable (``trainable=True``): the owners pull the halo
+  rows' gradients back the same way (``pna_halo_grad_pull``).
 * ``halo`` (``HaloAggregator``; the north star's wording, measured beside pull): the same rows through a pack kernel
   (``pna_gather_rows``) and ONE NCCL all-to-all-v (``torch.distributed.all_to_all_single``); rows whose sources are all
-  local can be reduced while the all-to-all is in flight (masked light views).
+  local can be reduced while the all-to-all is in flight (masked light views).  Needs only a process group, so it also
+  runs across nodes and between GPUs that cannot map each other's memory.  Trainable (``trainable=True``): the halo
+  rows' gradients go back through the transposed all-to-all and the owners add them with ``pna_halo_grad_pull``.
 * ``peer`` (``PeerAggregator``): ``col`` encodes ``owner << shift | row`` and the aggregation kernel gathers remote rows
   straight from the owner's HBM with the same asynchronous copies it uses for local rows -- gather and exchange are ONE
   kernel, no halo buffer at all; every remote EDGE crosses the link (peer lines are not cached in the local L2), so it
@@ -127,12 +129,66 @@ def gather_rows(src: torch.Tensor, idx: torch.Tensor, out: torch.Tensor) -> torc
     return out
 
 
-class HaloAggregator:
-    """[local ; halo] path: pack -> one NCCL all-to-all-v -> aggregation, interior rows overlapped with the exchange."""
+class _HaloExchange(torch.autograd.Function):
+    """x [n_local, F] -> a fresh [n_local + n_halo, F] tensor [x ; halo] (``agg.exchange_features``); the backward returns
+    the halo rows' gradients to their owners and gives back the fp32 gradient of x (``agg.return_halo_grad``)."""
 
-    def __init__(self, plan: HaloPlan, n_feat: int, dtype=torch.float32, group=None, overlap: bool = True):
+    @staticmethod
+    def forward(ctx, x, agg):
+        ctx.agg, ctx.x_dtype = agg, x.dtype
+        return agg.exchange_features(x)
+
+    @staticmethod
+    def backward(ctx, grad_ext):
+        return ctx.agg.return_halo_grad(grad_ext).to(ctx.x_dtype), None
+
+
+class _TrainableExchange:
+    """The differentiable aggregation shared by the planes with a backward.  A plane provides ``plan`` (n_local),
+    ``n_feat``, ``dtype``, ``csr`` over ``[local ; halo]``, ``trainable``, ``exchange_features(x)`` and
+    ``return_halo_grad(grad_ext)``."""
+
+    def _check_features(self, x: torch.Tensor) -> None:
+        n_local = self.plan.n_local
+        if tuple(x.shape) != (n_local, self.n_feat) or x.dtype != self.dtype:
+            raise ValueError(f"x must be [{n_local}, {self.n_feat}] {self.dtype}, got {tuple(x.shape)} {x.dtype}")
+
+    def pna_aggregate(self, x: torch.Tensor, aggregators, scalers, avg_deg, *, towers: int = 1,
+                      row_bias: Optional[torch.Tensor] = None, self_feat: Optional[torch.Tensor] = None,
+                      self_divided: bool = True, zero_isolated: bool = False, relu_var: bool = False,
+                      scaler_degree: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Differentiable aggregation of this rank's rows (``pna_b200.pna_aggregate`` on ``[x ; halo]``): x is the rank's
+        ``[n_local, F]`` features, ``row_bias`` / ``self_feat`` are per destination and stay local; returns the rank's
+        ``[n_local, width]`` output.  Every rank must make the same sequence of calls (each one exchanges the halo in the
+        forward and, if a gradient flows, returns it in the backward).  Gradients of parameters that produced ``x`` are
+        this rank's partial sums: all-reduce them across ranks before the optimizer step."""
+        if x.requires_grad and torch.is_grad_enabled() and not self.trainable:
+            raise RuntimeError(f"a gradient through the halo exchange needs {type(self).__name__}(..., trainable=True)")
+        x_ext = _HaloExchange.apply(x, self)
+        return pna_aggregate(x_ext, self.csr, aggregators, scalers, avg_deg, towers=towers, row_bias=row_bias,
+                             self_feat=self_feat, self_divided=self_divided, zero_isolated=zero_isolated, relu_var=relu_var,
+                             scaler_degree=scaler_degree)
+
+
+class HaloAggregator(_TrainableExchange):
+    """[local ; halo] path: pack -> one NCCL all-to-all-v -> aggregation, interior rows overlapped with the exchange.
+
+    Training (``trainable=True``; opt-in, a forward-only aggregator allocates and communicates nothing more):
+    ``pna_aggregate(x, ...)`` is differentiable in ``x``.  Forward: ``x`` into the head of a fresh ``[n_local + n_halo, F]``
+    tensor, pack, one all-to-all into its tail (the interior rows' overlap stays on the forward-only ``aggregate()``,
+    since the differentiable aggregation is one ``pna_aggregate`` over all rows).  Backward: the
+    transposed all-to-all sends every halo row's fp32 gradient back to its owner (``return_halo_grad``), which adds the
+    copies of a row into its own gradient in ascending peer rank with ``pna_halo_grad_pull``, without atomics: the
+    gradient return is bit-reproducible.  One fp32 receive buffer serves every layer; its reuse is ordered by the stream.
+    Parameter gradients are this rank's partial sums; summing them across ranks (``all_reduce``) is the caller's job.
+    ``_all_to_all`` replaces ``torch.distributed.all_to_all_single`` (same signature) in both directions: tests run W
+    ranks in one process through it."""
+
+    def __init__(self, plan: HaloPlan, n_feat: int, dtype=torch.float32, group=None, overlap: bool = True,
+                 trainable: bool = False, _all_to_all=None):
         dev = plan.src_ext.device
-        self.plan, self.group, self.overlap = plan, group, overlap
+        self.plan, self.group, self.overlap, self.n_feat, self.dtype = plan, group, overlap, n_feat, dtype
+        self._all_to_all = _all_to_all or dist.all_to_all_single
         self.csr = build_csr(plan.src_ext, plan.dst_local, plan.n_local, n_src=plan.n_local + plan.n_halo)
         self.x_ext = torch.zeros((plan.n_local + plan.n_halo, n_feat), dtype=dtype, device=dev)
         self.send_buf = torch.empty((int(plan.send_idx.numel()), n_feat), dtype=dtype, device=dev)
@@ -142,17 +198,64 @@ class HaloAggregator:
         if overlap:
             self.view_interior = self.csr.masked_view(plan.interior)
             self.view_boundary = self.csr.masked_view(~plan.interior)
+        # gradient return (trainable only): owner-side reverse plan, receive buffer, and per peer the start of its segment
+        self.trainable, self.grad_plan = trainable, None
+        self._grad_recv: Optional[torch.Tensor] = None
+        self._grad_table: Optional[torch.Tensor] = None
+        if trainable:
+            self.grad_plan = halo_grad_return_plan(plan)
+            self._grad_recv = torch.empty((int(plan.send_idx.numel()), n_feat), dtype=torch.float32, device=dev)
+            starts, off = [], 0
+            for n in plan.send_splits:
+                starts.append(self._grad_recv.data_ptr() + off * n_feat * 4)
+                off += n
+            self._grad_table = torch.tensor(starts, dtype=torch.int64, device=dev)
 
     @property
     def x_local(self) -> torch.Tensor:
         """The rank's own feature rows: produce the layer input in place here (head of the [local ; halo] buffer)."""
         return self.x_ext[: self.plan.n_local]
 
-    def exchange(self) -> None:
+    def _exchange_into(self, x_ext: torch.Tensor) -> None:
         p = self.plan
-        gather_rows(self.x_local, p.send_idx, self.send_buf)
-        dist.all_to_all_single(self.x_ext[p.n_local:], self.send_buf, output_split_sizes=p.recv_splits,
-                               input_split_sizes=p.send_splits, group=self.group)
+        gather_rows(x_ext[:p.n_local], p.send_idx, self.send_buf)
+        self._all_to_all(x_ext[p.n_local:], self.send_buf, output_split_sizes=p.recv_splits,
+                         input_split_sizes=p.send_splits, group=self.group)
+
+    def exchange(self) -> None:
+        self._exchange_into(self.x_ext)
+
+    # ---- differentiable path (trainable=True) ----
+    def exchange_features(self, x: torch.Tensor) -> torch.Tensor:
+        """Forward half of the differentiable exchange, without autograd: a fresh ``[n_local + n_halo, F]`` tensor
+        ``[x ; halo]``, its tail filled by pack + all-to-all."""
+        p = self.plan
+        self._check_features(x)
+        x_ext = torch.empty((p.n_local + p.n_halo, self.n_feat), dtype=self.dtype, device=x.device)
+        x_ext[:p.n_local].copy_(x)
+        self._exchange_into(x_ext)
+        return x_ext
+
+    def return_halo_grad(self, grad_ext: torch.Tensor) -> torch.Tensor:
+        """Backward of the exchange: this rank's fp32 gradient for its halo rows goes back to their owners (the forward
+        all-to-all with the split sizes swapped; the halo is grouped by owner, so nothing is packed); returns a fp32 copy of
+        ``grad_ext[:n_local]`` plus the gradients every peer returned for copies of this rank's rows
+        (``pna_halo_grad_pull``, its pointer table aimed at the peers' segments of the local receive buffer)."""
+        p, gp = self.plan, self.grad_plan
+        if not self.trainable:
+            raise RuntimeError("the gradient return needs HaloAggregator(..., trainable=True)")
+        send = grad_ext[p.n_local:p.n_local + p.n_halo].to(torch.float32).contiguous()
+        self._all_to_all(self._grad_recv, send, output_split_sizes=p.send_splits, input_split_sizes=p.recv_splits,
+                         group=self.group)
+        dev = self._grad_recv.device
+        g = torch.empty((p.n_local, self.n_feat), dtype=torch.float32, device=dev)
+        g.copy_(grad_ext[:p.n_local])
+        if gp.n_rows:
+            with torch.cuda.device(dev):
+                _lib.check(_lib.lib().pna_halo_grad_pull(self._grad_table.data_ptr(), self.n_feat, gp.rows.data_ptr(),
+                                                         gp.rowptr.data_ptr(), gp.enc.data_ptr(), gp.shift, gp.n_rows, g.data_ptr(),
+                                                         self.n_feat, self.n_feat, torch.cuda.current_stream(dev).cuda_stream))
+        return g
 
     def aggregate(self, aggregators, scalers, avg_deg, out: Optional[torch.Tensor] = None, **kw) -> torch.Tensor:
         main = torch.cuda.current_stream(self.x_ext.device)
@@ -202,19 +305,21 @@ def build_pull_plan(src_global: torch.Tensor, dst_global: torch.Tensor, bounds: 
     return PullPlan(rank, world, lo, hi, n_local, n_halo, shift, src_ext, dst_global - lo, halo_ids, enc, int(remote.sum()))
 
 
-# ---- the pull plane's backward: return halo gradients to their owners -------------------------------------------------
+# ---- backward of the pull and halo planes: return halo gradients to their owners --------------------------------------
 @dataclass
 class GradReturnPlan:
-    """The owner's side of the pull plane's backward: which of this rank's rows its peers hold as halo copies, and where.
-    A compact CSR over the rows that have at least one copy; the slots of a row are in ascending peer rank, so
-    ``pna_halo_grad_pull`` adds them in a fixed order."""
+    """The owner's side of the backward: which of this rank's rows its peers hold as halo copies, and where their
+    gradients arrive.  A compact CSR over the rows that have at least one copy; the slots of a row are in ascending peer
+    rank, so ``pna_halo_grad_pull`` adds them in a fixed order."""
     rank: int
     world: int
-    shift: int                     # enc = peer << shift | position in that peer's halo
+    shift: int                     # enc = peer << shift | position in that peer's segment
     rows: torch.Tensor             # int32 [n_rows] local rows held by at least one peer, ascending
     rowptr: torch.Tensor           # int32 [n_rows + 1]
     enc: torch.Tensor              # int32 [rowptr[-1]]
-    peer_n_local: List[int]        # every rank's n_local: where its halo-gradient rows start in its [local ; halo] buffer
+    # pull plane only: every rank's n_local, where its halo-gradient rows start in its [local ; halo] buffer.  None in the
+    # halo plane's plan (halo_grad_return_plan), whose segments are the peers' parts of the local receive buffer.
+    peer_n_local: Optional[List[int]] = None
 
     @property
     def n_rows(self) -> int:
@@ -230,13 +335,14 @@ def grad_return_shift(max_halo: int, world: int) -> int:
 
 
 def grad_return_plan(rank: int, world: int, held: List[torch.Tensor], offsets: List[int], max_halo: int,
-                     peer_n_local: List[int], device=None) -> GradReturnPlan:
+                     peer_n_local: Optional[List[int]] = None, device=None) -> GradReturnPlan:
     """Owner ``rank``'s reverse plan from per-peer lists (pure; no communication).
 
     held[p]   : int64, this rank's rows (owner-local ids, ascending) that rank p holds in its halo;
-    offsets[p]: position of the first of them in p's halo (p's halo ids are sorted, hence grouped by owner, so this rank's
-                rows are one contiguous segment of it and row held[p][i] sits at offsets[p] + i);
-    max_halo  : the largest n_halo of any rank -- it sizes the position field of the encoding."""
+    offsets[p]: position of the first of them in p's segment (pull plane: p's halo, whose ids are sorted, hence grouped by
+                owner, so this rank's rows are one contiguous segment of it and row held[p][i] sits at offsets[p] + i);
+    max_halo  : the largest position + 1 any slot can have -- it sizes the position field of the encoding;
+    peer_n_local: every rank's n_local, which only the pull plane reads (``PullAggregator``)."""
     shift = grad_return_shift(max_halo, world)
     if device is None:
         device = held[0].device if held else torch.device("cpu")
@@ -250,18 +356,28 @@ def grad_return_plan(rank: int, world: int, held: List[torch.Tensor], offsets: L
         pos = int(offsets[p]) + torch.arange(ids.numel(), dtype=torch.int64, device=device)
         rows_l.append(ids)
         enc_l.append((p << shift) | pos)
+    n_local = None if peer_n_local is None else list(map(int, peer_n_local))
     if not rows_l:
         empty = torch.zeros(0, dtype=torch.int32, device=device)
         return GradReturnPlan(rank, world, shift, empty, torch.zeros(1, dtype=torch.int32, device=device), empty.clone(),
-                              list(map(int, peer_n_local)))
+                              n_local)
     rows, enc = torch.cat(rows_l), torch.cat(enc_l)
     order = torch.sort(rows, stable=True).indices          # peers were appended in rank order: stable keeps it per row
     rows, enc = rows[order], enc[order]
     uniq, counts = torch.unique_consecutive(rows, return_counts=True)
     rowptr = torch.zeros(uniq.numel() + 1, dtype=torch.int64, device=device)
     rowptr[1:] = torch.cumsum(counts, 0)
-    return GradReturnPlan(rank, world, shift, uniq.to(torch.int32), rowptr.to(torch.int32), enc.to(torch.int32),
-                          list(map(int, peer_n_local)))
+    return GradReturnPlan(rank, world, shift, uniq.to(torch.int32), rowptr.to(torch.int32), enc.to(torch.int32), n_local)
+
+
+def halo_grad_return_plan(plan: HaloPlan) -> GradReturnPlan:
+    """The halo plane's reverse plan, from the owner's own ``HaloPlan`` (pure, local; no collective).  In the backward,
+    peer p returns the gradients of the rows this rank sent it, in the order it sent them: the owner's receive buffer holds
+    p's segment at ``send_off[p]``, and position ``send_off[p] + q`` carries the gradient of local row
+    ``send_idx[send_off[p] + q]``.  Slot encoding: ``p << shift | q``, q < send_splits[p]."""
+    held = list(torch.split(plan.send_idx.to(torch.int64), plan.send_splits))
+    return grad_return_plan(plan.rank, plan.world, held, [0] * plan.world, max(plan.send_splits, default=0),
+                            device=plan.send_idx.device)
 
 
 def _halo_segments(plan: PullPlan):
@@ -310,23 +426,7 @@ def build_grad_return_plan(plan: PullPlan, group=None) -> GradReturnPlan:
                             device=dev)
 
 
-class _HaloExchange(torch.autograd.Function):
-    """x [n_local, F] -> a fresh [n_local + n_halo, F] copy of [x ; halo]; backward returns the halo rows' gradients to
-    their owners (``PullAggregator.stage_halo_grad`` + ``pull_halo_grad``)."""
-
-    @staticmethod
-    def forward(ctx, x, agg):
-        ctx.agg, ctx.x_dtype = agg, x.dtype
-        return agg.exchange_features(x)
-
-    @staticmethod
-    def backward(ctx, grad_ext):
-        agg = ctx.agg
-        agg.stage_halo_grad(grad_ext)
-        return agg.pull_halo_grad(grad_ext).to(ctx.x_dtype), None
-
-
-class PullAggregator:
+class PullAggregator(_TrainableExchange):
     """[local ; halo] source buffer whose halo tail is filled by ONE kernel of peer loads (``pna_halo_pull``): the
     all-to-all of the north star without a collective -- no id exchange when the graph is planned, no pack kernel, no
     send buffer, no NCCL call per layer; a remote row crosses NVLink once per layer however often it is gathered.
@@ -379,6 +479,8 @@ class PullAggregator:
                     plan.rank, 1, [torch.zeros(0, dtype=torch.int64, device=dev)], [0], plan.n_halo, [plan.n_local], device=dev)
             if grad_plan.rank != plan.rank or grad_plan.world != plan.world:
                 raise ValueError("grad_plan belongs to another rank or world")
+            if grad_plan.peer_n_local is None:
+                raise ValueError("grad_plan has no peer_n_local: it is not a pull-plane reverse plan")
             self.grad_plan = grad_plan
             for _ in range(buffers):
                 t, ptrs, keep = alloc((int(rows), n_feat), torch.float32)
@@ -436,9 +538,7 @@ class PullAggregator:
     def exchange_features(self, x: torch.Tensor) -> torch.Tensor:
         """Forward half of the differentiable exchange, without autograd: ``x`` -> ``x_local``, barrier, pull; returns a
         fresh ``[n_local + n_halo, F]`` copy of ``[x ; halo]`` and flips to the other feature buffer."""
-        p = self.plan
-        if tuple(x.shape) != (p.n_local, self.n_feat) or x.dtype != self.dtype:
-            raise ValueError(f"x must be [{p.n_local}, {self.n_feat}] {self.dtype}, got {tuple(x.shape)} {x.dtype}")
+        self._check_features(x)
         self.x_local.copy_(x)
         self.exchange()
         out = self.x_ext.clone()
@@ -473,21 +573,10 @@ class PullAggregator:
         self._gcur = (self._gcur + 1) % len(self._gbufs)
         return g
 
-    def pna_aggregate(self, x: torch.Tensor, aggregators, scalers, avg_deg, *, towers: int = 1,
-                      row_bias: Optional[torch.Tensor] = None, self_feat: Optional[torch.Tensor] = None,
-                      self_divided: bool = True, zero_isolated: bool = False, relu_var: bool = False,
-                      scaler_degree: Optional[torch.Tensor] = None) -> torch.Tensor:
-        """Differentiable aggregation of this rank's rows (``pna_b200.pna_aggregate`` on ``[x ; halo]``): x is the rank's
-        ``[n_local, F]`` features, ``row_bias`` / ``self_feat`` are per destination and stay local; returns the rank's
-        ``[n_local, width]`` output.  Every rank must make the same sequence of calls (each one holds a barrier in the
-        forward and, if a gradient flows, one in the backward).  Gradients of parameters that produced ``x`` are
-        this rank's partial sums: all-reduce them across ranks before the optimizer step."""
-        if x.requires_grad and torch.is_grad_enabled() and not self.trainable:
-            raise RuntimeError("a gradient through the halo exchange needs PullAggregator(..., trainable=True)")
-        x_ext = _HaloExchange.apply(x, self)
-        return pna_aggregate(x_ext, self.csr, aggregators, scalers, avg_deg, towers=towers, row_bias=row_bias,
-                             self_feat=self_feat, self_divided=self_divided, zero_isolated=zero_isolated, relu_var=relu_var,
-                             scaler_degree=scaler_degree)
+    def return_halo_grad(self, grad_ext: torch.Tensor) -> torch.Tensor:
+        """Backward of the exchange: ``stage_halo_grad`` then ``pull_halo_grad`` (one barrier)."""
+        self.stage_halo_grad(grad_ext)
+        return self.pull_halo_grad(grad_ext)
 
     def check(self) -> None:
         """Host-side check (synchronises): did every barrier see all peers arrive?"""
