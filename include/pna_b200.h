@@ -333,6 +333,35 @@ int pna_linear_fwd(const float* a, int64_t lda, const float* weight, const float
 int pna_linear_scaled_fwd(const float* a, int64_t lda, const float* row_scale, int32_t n_scalers, const float* weight,
                           const float* bias, float* y, int64_t ldy, int64_t n_rows, int32_t n_in, int32_t n_out, void* workspace,
                           size_t workspace_bytes, pna_stream_t stream);
+
+/* ---- backward of pna_linear_fwd / pna_linear_scaled_fwd on the tensor cores, at the same fp32 accuracy (3xTF32) -----
+ * Both calls are deterministic: no atomics, every sum in a fixed order, so the result is a fixed function of the inputs
+ * (what torch.use_deterministic_algorithms promises).  n_scalers == 1 with row_scale NULL is the plain linear; otherwise
+ * row_scale is the [n_rows, n_scalers] contiguous factor array of pna_linear_scaled_fwd and n_a = n_in / n_scalers.  Shapes
+ * as the forward's: n_a % 32 == 0 and n_out in {64, 128, 256} (else PNA_ERR_UNSUPPORTED); n_scalers outside 1..5, null
+ * pointers, or row_scale NULL with n_scalers > 1: PNA_ERR_BAD_ARG.  grad_y, a, grad_a, grad_weight and workspace 16-byte
+ * aligned, row pitches (in elements) multiples of 4.  n_rows == 0 returns PNA_OK and launches nothing.
+ *
+ * Data gradient, grad_a [n_rows, n_a] (pitch ld_grad_a) written:
+ *     grad_a[i, k] = sum_s sum_o  fl(row_scale[i, s] * grad_y[i, o]) * weight[o, s * n_a + k]
+ * (plain: sum_o grad_y[i, o] * weight[o, k]).  The forward kernel run on grad_y with the transposed (and, with scalers,
+ * re-blocked) weight; the scaled copies of grad_y exist only in registers.
+ * Weight gradient, grad_weight [n_out, n_in] contiguous written (not accumulated):
+ *     grad_weight[o, s * n_a + k] = sum_i  grad_y[i, o] * fl(row_scale[i, s] * a[i, k])
+ * where fl(c * a) is the operand the forward's loaders formed, so this is the exact gradient of what the forward multiplied.
+ * The rows are split across CTAs by a rule that depends on the shape alone; each CTA folds its tensor-core accumulators
+ * into an fp32 partial every 64 rows and a second kernel adds the partials in ascending split order.  grad_a folds the
+ * same way every 128 products.
+ * workspace: pna_linear_bwd_workspace_bytes(n_rows, n_in, n_out, n_scalers) bytes, enough for either call (the weight
+ * images of the data gradient, the partials of the weight gradient); calls on one stream may share it. */
+int pna_linear_bwd_workspace_bytes(int64_t n_rows, int32_t n_in, int32_t n_out, int32_t n_scalers, size_t* bytes);
+int pna_linear_bwd_data(const float* grad_y, int64_t ld_grad_y, const float* row_scale, int32_t n_scalers, const float* weight,
+                        float* grad_a, int64_t ld_grad_a, int64_t n_rows, int32_t n_in, int32_t n_out, void* workspace,
+                        size_t workspace_bytes, pna_stream_t stream);
+int pna_linear_bwd_weight(const float* grad_y, int64_t ld_grad_y, const float* a, int64_t lda, const float* row_scale,
+                          int32_t n_scalers, float* grad_weight, int64_t n_rows, int32_t n_in, int32_t n_out, void* workspace,
+                          size_t workspace_bytes, pna_stream_t stream);
+
 /* scales[i, s] = factor of scaler s (code (scaler_codes >> 4s) & 15) at in-degree rowptr[i+1] - rowptr[i]; bit-identical
  * to the factors pna_aggregate_fwd applies (one device function computes both). */
 int pna_row_scales(const int32_t* rowptr, int64_t n_rows, int32_t n_scalers, uint32_t scaler_codes, float avg_log, float avg_lin,

@@ -39,7 +39,8 @@ FLAG_ZERO_ISOLATED, FLAG_SKIP_LIGHT, FLAG_SKIP_HUBS, FLAG_RELU_VAR, FLAG_GATHER_
 # every symbol the header declares (checked by tests/test_abi.py)
 EXPORTED_SYMBOLS = ("pna_csr_workspace_bytes", "pna_csr_build", "pna_csr_light_view", "pna_csr_light_view_workspace_bytes", "pna_aggregate_fwd", "pna_aggregate_bwd",
                     "pna_aggregate_bwd_coef", "pna_aggregate_bwd_combine", "pna_aggregate_bwd_slots",
-                    "pna_gather_rows", "pna_halo_pull", "pna_halo_grad_pull", "pna_peer_barrier", "pna_linear_fwd", "pna_linear_scaled_fwd", "pna_row_scales", "pna_linear_workspace_bytes", "pna_query", "pna_last_error")
+                    "pna_gather_rows", "pna_halo_pull", "pna_halo_grad_pull", "pna_peer_barrier", "pna_linear_fwd", "pna_linear_scaled_fwd", "pna_row_scales", "pna_linear_workspace_bytes",
+                    "pna_linear_bwd_workspace_bytes", "pna_linear_bwd_data", "pna_linear_bwd_weight", "pna_query", "pna_last_error")
 
 
 class PnaError(RuntimeError):
@@ -187,6 +188,14 @@ def lib() -> C.CDLL:
         L.pna_linear_scaled_fwd.restype = C.c_int
         L.pna_linear_scaled_fwd.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                             C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]
+        L.pna_linear_bwd_workspace_bytes.restype = C.c_int
+        L.pna_linear_bwd_workspace_bytes.argtypes = [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_size_t)]
+        L.pna_linear_bwd_data.restype = C.c_int
+        L.pna_linear_bwd_data.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,
+                                          C.c_int32, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]
+        L.pna_linear_bwd_weight.restype = C.c_int
+        L.pna_linear_bwd_weight.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64,
+                                            C.c_int32, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]
         L.pna_row_scales.restype = C.c_int
         L.pna_row_scales.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_uint32, C.c_float, C.c_float, C.c_void_p, C.c_void_p]
         abi = L.pna_query(QUERY_ABI_VERSION)

@@ -25,6 +25,11 @@
 // fl(c_s(i) * a) rounded exactly like the reference's multiply, right before the hi/lo split -- the [N, S*A*F] tensor
 // never exists in HBM: the aggregation writes, and this kernel reads, 1/S of the bytes.  K blocks are visited
 // compact-block-major, scaler-minor; the W tile of step (kb, s) is block s * (K/32) + kb of the reference's weight.
+//
+// Backward -- pna_linear_bwd_data / pna_linear_bwd_weight, at the same fp32 accuracy and deterministic (no atomics):
+// dA runs the kernel above on dY with the transposed weight in column slabs; dW is k_linear_bwd_weight (below).
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace pna {
@@ -81,24 +86,25 @@ __device__ __forceinline__ unsigned long long lin_desc(unsigned smem_addr) {
 #define LIN_F16(a, i) LIN_F4(a, i), LIN_F4(a, i + 4), LIN_F4(a, i + 8), LIN_F4(a, i + 12)
 
 // D[64 x N] += A[64 x 8] . B[N x 8]^T, tf32 operands from shared memory, fp32 accumulator in registers (N/2 per thread:
-// register 4j + q of lane l holds row l/4 + 8 (q/2) of the warp's 16 rows, column 8j + 2 (l%4) + q%2)
+// register 4j + q of lane l holds row l/4 + 8 (q/2) of the warp's 16 rows, column 8j + 2 (l%4) + q%2).  add == 0: D = A . B
+// (restarts an accumulation chain without writing the registers outside the MMA pipeline)
 template <int N>
-__device__ __forceinline__ void lin_wgmma(float (&d)[N / 2], unsigned long long adesc, unsigned long long bdesc);
+__device__ __forceinline__ void lin_wgmma(float (&d)[N / 2], unsigned long long adesc, unsigned long long bdesc, int add = 1);
 template <>
-__device__ __forceinline__ void lin_wgmma<64>(float (&d)[32], unsigned long long adesc, unsigned long long bdesc) {
+__device__ __forceinline__ void lin_wgmma<64>(float (&d)[32], unsigned long long adesc, unsigned long long bdesc, int add) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {"
       "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
       "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
       "}, %32, %33, p, 1, 1;\n\t}"
       : LIN_F16(d, 0), LIN_F16(d, 16)
-      : "l"(adesc), "l"(bdesc));
+      : "l"(adesc), "l"(bdesc), "r"(add));
 }
 template <>
-__device__ __forceinline__ void lin_wgmma<128>(float (&d)[64], unsigned long long adesc, unsigned long long bdesc) {
+__device__ __forceinline__ void lin_wgmma<128>(float (&d)[64], unsigned long long adesc, unsigned long long bdesc, int add) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {"
       "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
       "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
@@ -106,7 +112,7 @@ __device__ __forceinline__ void lin_wgmma<128>(float (&d)[64], unsigned long lon
       "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
       "}, %64, %65, p, 1, 1;\n\t}"
       : LIN_F16(d, 0), LIN_F16(d, 16), LIN_F16(d, 32), LIN_F16(d, 48)
-      : "l"(adesc), "l"(bdesc));
+      : "l"(adesc), "l"(bdesc), "r"(add));
 }
 // keeps the compiler from moving accumulator registers across the asynchronous MMAs
 template <int R>
@@ -131,20 +137,34 @@ struct LinSmem {
 
 // Wimg: for every K block the exact shared-memory images of the W hi and W lo tiles ([O rows][128 B], swizzled),
 // produced once per call by k_split_weight -- so a tile is ONE contiguous bulk copy (TMA 1-D, no tensor map needed).
-template <int O>
+// Column slabs (the data gradient, whose width n_cols is not an O of its own): CTA b computes the O columns of slab
+// b % n_slabs of row tile b / n_slabs -- the slabs of one row tile run side by side and read its A rows from L2 -- with
+// the slab's own weight image (n_it K blocks each, zero rows past n_cols); stores to columns >= n_cols are dropped.
+// The forward is n_slabs = 1, n_cols = O.
+// FOLD (the data gradient): every kLinFoldSteps pipeline steps the warps wait for their MMAs and fold (acc + corr) into the
+// CTA's own Y tile (stored the first time, added with one round-to-nearest add after), so no truncating tensor-core
+// accumulation chain is longer than kLinFoldSteps * 32 products: with the S scalers the chain would be S * O long.
+// (ptxas serializes this instance's wgmmas -- it cannot see that the accumulators are read only after a full drain -- so
+// pna_linear_bwd_data launches it only where a fold happens.)
+constexpr int kLinFoldSteps = 4;
+template <int O, bool FOLD = false>
 __global__ void __launch_bounds__(kLinThreads, 1)
 k_linear_3xtf32(const float* __restrict__ A, long long lda, const float* __restrict__ row_scale, int n_rep,
                 const float* __restrict__ Wimg, const float* __restrict__ bias, float* __restrict__ Y, long long ldy, long long N,
-                int K) {
+                int K, int n_slabs, int n_cols) {
   constexpr int kSt = LinSmem<O>::kSt, kM = LinSmem<O>::kM, kN = LinSmem<O>::kN;
   extern __shared__ unsigned char lin_raw[];
   const unsigned base = (lin_smem_u32(lin_raw) + 1023u) & ~1023u;          // swizzle atoms need 1024-byte alignment
   unsigned char* gbase = lin_raw + (base - lin_smem_u32(lin_raw));
   const unsigned bars = base + kSt * LinSmem<O>::kStage;                    // full[kSt], empty[kSt]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const long long row0 = (long long)blockIdx.x * kM;
+  const int slab = (int)(blockIdx.x % (unsigned)n_slabs);
+  const long long row0 = (long long)(blockIdx.x / (unsigned)n_slabs) * kM;
   const int n_kb = K / kLinBK;          // K blocks of A (compact width)
   const int n_it = n_kb * n_rep;        // pipeline steps = K blocks of W (n_rep == 1 without row scales)
+  Wimg += (long long)slab * n_it * (2 * O * kLinBK);
+  Y += (long long)slab * O;
+  const int c_end = n_cols - slab * O;  // columns of this slab that exist
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kSt; ++s) {
@@ -182,6 +202,31 @@ k_linear_3xtf32(const float* __restrict__ A, long long lda, const float* __restr
     float acc[kN / 2], corr[kN / 2];
 #pragma unroll
     for (int i = 0; i < kN / 2; ++i) { acc[i] = 0.f; corr[i] = 0.f; }
+    // ---------------- epilogue: (main + cross terms) + bias, two adjacent columns per store (FOLD: + the Y tile so far) -----
+    const int wr = (warp & 3) * 16 + (lane >> 2);           // row of the warpgroup's 64 for registers 4j, 4j + 1
+    const long long r_lo = row0 + (O <= 128 ? wg * 64 : 0) + wr, r_hi = r_lo + 8;
+    bool folded = false, restart = false;
+    auto emit = [&](const float* bs, bool add) {
+#pragma unroll
+      for (int jj = 0; jj < kN / 8; ++jj) {
+        const int c = (O <= 128 ? 0 : wg * kN) + jj * 8 + 2 * (lane & 3);
+        if (c >= c_end) continue;
+        const float b0 = bs ? __ldg(bs + c) : 0.f, b1 = bs ? __ldg(bs + c + 1) : 0.f;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const long long r = h ? r_hi : r_lo;
+          if (r >= N) continue;
+          float2* p = reinterpret_cast<float2*>(Y + r * ldy + c);
+          float2 v = make_float2((acc[4 * jj + 2 * h] + corr[4 * jj + 2 * h]) + b0,
+                                  (acc[4 * jj + 2 * h + 1] + corr[4 * jj + 2 * h + 1]) + b1);
+          if (FOLD && add) {
+            const float2 old = *p;
+            v.x = old.x + v.x; v.y = old.y + v.y;
+          }
+          *p = v;
+        }
+      }
+    };
     float4 pre[kAhead][kSlabs];
     auto fetch = [&](int kb, float4 (&dst)[kSlabs]) {
 #pragma unroll
@@ -242,13 +287,22 @@ k_linear_3xtf32(const float* __restrict__ A, long long lda, const float* __restr
 #pragma unroll
           for (int ks = 0; ks < kLinBK / 8; ++ks) {         // K = 8 tf32 = 32 bytes along the swizzled row
             const unsigned ko = ks * 32;
-            lin_wgmma<kN>(corr, lin_desc(a_hi + ko), lin_desc(w_lo + ko));
+            const int add = FOLD ? (ks > 0 || !restart) : 1;  // FOLD: the first MMAs after a fold start a new chain
+            lin_wgmma<kN>(corr, lin_desc(a_hi + ko), lin_desc(w_lo + ko), add);
             lin_wgmma<kN>(corr, lin_desc(a_lo + ko), lin_desc(w_hi + ko));
-            lin_wgmma<kN>(acc, lin_desc(a_hi + ko), lin_desc(w_hi + ko));
+            lin_wgmma<kN>(acc, lin_desc(a_hi + ko), lin_desc(w_hi + ko), add);
           }
+          restart = false;
           asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
-          asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");     // the previous step's MMAs are done
-          lin_fence_acc(acc); lin_fence_acc(corr);
+          if (FOLD && (it + 1) % kLinFoldSteps == 0 && it + 1 < n_it) {
+            asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");   // this step's too: fold the chain
+            lin_fence_acc(acc); lin_fence_acc(corr);
+            emit(nullptr, folded);
+            folded = restart = true;
+          } else {
+            asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");   // the previous step's MMAs are done
+            lin_fence_acc(acc); lin_fence_acc(corr);
+          }
           if (prev >= 0) {
             if (lane == 0) lin_mbar_arrive(bars + 8 * (kSt + prev));
             const int t = it - 1 + kSt;                     // the next step that uses the released stage
@@ -266,19 +320,7 @@ k_linear_3xtf32(const float* __restrict__ A, long long lda, const float* __restr
     }
     asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
     lin_fence_acc(acc); lin_fence_acc(corr);
-    // ---------------- epilogue: (main + cross terms) + bias, two adjacent columns per store ----------------
-    const int wr = (warp & 3) * 16 + (lane >> 2);           // row of the warpgroup's 64 for registers 4j, 4j + 1
-    const long long r_lo = row0 + (O <= 128 ? wg * 64 : 0) + wr, r_hi = r_lo + 8;
-#pragma unroll
-    for (int jj = 0; jj < kN / 8; ++jj) {
-      const int c = (O <= 128 ? 0 : wg * kN) + jj * 8 + 2 * (lane & 3);
-      const float b0 = bias ? __ldg(bias + c) : 0.f, b1 = bias ? __ldg(bias + c + 1) : 0.f;
-      if (r_lo < N)
-        *reinterpret_cast<float2*>(Y + r_lo * ldy + c) = make_float2((acc[4 * jj] + corr[4 * jj]) + b0, (acc[4 * jj + 1] + corr[4 * jj + 1]) + b1);
-      if (r_hi < N)
-        *reinterpret_cast<float2*>(Y + r_hi * ldy + c) =
-            make_float2((acc[4 * jj + 2] + corr[4 * jj + 2]) + b0, (acc[4 * jj + 3] + corr[4 * jj + 3]) + b1);
-    }
+    emit(bias, FOLD && folded);
   }
 }
 
@@ -301,17 +343,277 @@ __global__ void k_split_weight(const float* __restrict__ W, int O, int K, float*
   *reinterpret_cast<float4*>(tile + O * kLinBK + off) = lo;
 }
 
-template <int O>
+template <int O, bool FOLD = false>
 static int launch_linear(const float* A, long long lda, const float* row_scale, int n_rep, const float* Wimg, const float* bias,
-                         float* Y, long long ldy, long long N, int K, cudaStream_t st) {
-  auto kern = k_linear_3xtf32<O>;
+                         float* Y, long long ldy, long long N, int K, cudaStream_t st, int n_slabs = 1, int n_cols = O) {
+  auto kern = k_linear_3xtf32<O, FOLD>;
   static bool attr_set = false;
   if (!attr_set) {
     PNA_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LinSmem<O>::kBytes));
     attr_set = true;
   }
-  const long long grid = (N + LinSmem<O>::kM - 1) / LinSmem<O>::kM;
-  kern<<<(unsigned)grid, kLinThreads, LinSmem<O>::kBytes, st>>>(A, lda, row_scale, n_rep, Wimg, bias, Y, ldy, N, K);
+  const long long grid = (N + LinSmem<O>::kM - 1) / LinSmem<O>::kM * n_slabs;
+  kern<<<(unsigned)grid, kLinThreads, LinSmem<O>::kBytes, st>>>(A, lda, row_scale, n_rep, Wimg, bias, Y, ldy, N, K, n_slabs, n_cols);
+  PNA_CUDA_TRY(cudaGetLastError());
+  return PNA_OK;
+}
+
+// ================================ backward (pna_linear_bwd_data / pna_linear_bwd_weight) ================================
+//
+// Data gradient: k_linear_3xtf32 with A = dY (K = O) and the weight W''[c, s * O + o] = W[o, s * n_cols + c]
+// (n_cols = n_in / S), in column slabs of width Os.  With row scales the loaders form fl(c_s(i) * dY) like the forward's.
+
+// slab width for n_cols output columns: 128, or 64 where that pads less (n_cols % 128 in (0, 64]).  Never 256: rounding
+// up to 256 never pads less than rounding up to 128, and O = 256's 64-row tiles double the weight traffic per output.
+static int bwd_data_slab(int n_cols) {
+  return (n_cols + 63) / 64 * 64 < (n_cols + 127) / 128 * 128 ? 64 : 128;
+}
+
+// W [O, n_in] -> per slab of Os columns of W'' and per K block of W'' the swizzled hi / lo images (as k_split_weight)
+__global__ void k_split_weight_t(const float* __restrict__ W, int O, int n_in, int n_rep, int Os, int n_slabs,
+                                 float* __restrict__ img) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;    // one 16-byte unit of the image
+  const int n_cols = n_in / n_rep, n_kbw = O * n_rep / kLinBK;
+  if (i >= (long long)n_slabs * n_kbw * 8 * Os) return;
+  const int r = (int)(i % Os);                      // consecutive threads: consecutive columns of W, coalesced reads
+  const long long t = i / Os;
+  const int j = (int)(t % 8), kbw = (int)(t / 8 % n_kbw), slab = (int)(t / 8 / n_kbw);
+  const int c = slab * Os + r;
+  const int kk = kbw * kLinBK + j * 4;              // first W'' column of the unit; O % 32 == 0: one scaler per unit
+  const int s = kk / O, o = kk % O;
+  float v[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) v[e] = c < n_cols ? __ldg(W + (long long)(o + e) * n_in + s * n_cols + c) : 0.f;
+  float4 hi, lo;
+  hi.x = lin_tf32(v[0]); lo.x = lin_tf32(v[0] - hi.x);
+  hi.y = lin_tf32(v[1]); lo.y = lin_tf32(v[1] - hi.y);
+  hi.z = lin_tf32(v[2]); lo.z = lin_tf32(v[2] - hi.z);
+  hi.w = lin_tf32(v[3]); lo.w = lin_tf32(v[3] - hi.w);
+  float* tile = img + ((long long)slab * n_kbw + kbw) * (2 * Os * kLinBK);
+  const unsigned off = lin_swz(r, j) / 4;
+  *reinterpret_cast<float4*>(tile + off) = hi;
+  *reinterpret_cast<float4*>(tile + Os * kLinBK + off) = lo;
+}
+
+// Weight gradient dW[o, c] = sum_i dY[i, o] . a'[i, c]  (a' = a, or fl(row_scale[i, c / n_a] * a[i, c % n_a])).
+// The reduction runs over the ROWS of both operands and tf32 wgmma reads K-major operands only, so the loaders transpose:
+// a thread loads a 4-row x 4-column block (four coalesced 16-byte loads), splits it hi / lo and stores its four columns as
+// four 16-byte K-major units (row = column of the operand, unit = its 4 rows) into the 128-byte-swizzled tiles; the 8
+// threads of a quarter-warp hold the 8 units of one swizzled row, so the stores are conflict free.
+// CTA tile: kTO outputs (rows of dW) x 128 columns, two warpgroups of 64 x kN.  A CTA owns one split of the rows; every
+// kWgFoldRows rows it waits for its MMAs and folds (acc + corr) into an fp32 partial in shared memory (each thread its own
+// words) with one round-to-nearest add, so no tensor-core accumulation chain (truncating adds) is longer than
+// kWgFoldRows / 8 steps; the partial goes to HBM once at the end.  No atomics: it is stored into the CTA's own tile of the
+// workspace (or into dW itself with one split), and k_sum_splits adds the splits in ascending order.
+constexpr int kWgFoldRows = 64;
+constexpr int kWgMinSplitRows = 512;
+constexpr int kWgTargetCtas = 264;    // two waves of H100 SXM's 132 SMs at one CTA per SM
+constexpr int kWgAhead = 2;           // K blocks of operands in flight per thread
+
+template <int O>
+struct WgSmem {
+  static constexpr int kTO = O <= 128 ? O : 128;          // dW rows per CTA (O = 256: two tiles)
+  static constexpr int kTC = 128;                          // dW columns per CTA
+  static constexpr int kN = O == 64 ? 64 : 128;            // columns per warpgroup (O = 64: the warpgroups split columns)
+  static constexpr int kYTile = kTO * 128, kATile = kTC * 128;
+  static constexpr int kStage = 2 * kYTile + 2 * kATile;   // dY hi, dY lo, a hi, a lo
+  static constexpr int kSt = 2;
+  static constexpr int kPart = kTO * kTC * 4;               // the fp32 partial tile
+  static constexpr int kBlocks = 2 * kTO + 2 * kTC;        // 4 x 4 blocks of a 32-row K block (dY, then a)
+  static constexpr int kPer = (kBlocks + kLinThreads - 1) / kLinThreads;
+  static constexpr size_t kBytes = 1024 /*align slack*/ + (size_t)kSt * kStage + kPart;
+};
+
+struct BwdWeightPlan {
+  int col_tiles, o_tiles, n_split;
+  long long rows;                     // rows per split, a multiple of 32
+};
+// depends on the shape alone (not on the device), so the partials -- and the bits of dW -- do too
+static BwdWeightPlan bwd_weight_plan(long long n_rows, int n_in, int n_out) {
+  BwdWeightPlan p;
+  p.col_tiles = (n_in + 127) / 128;
+  p.o_tiles = n_out > 128 ? 2 : 1;
+  const long long tiles = (long long)p.col_tiles * p.o_tiles;
+  long long sp = std::min((n_rows + kWgMinSplitRows - 1) / kWgMinSplitRows, std::max(1ll, (kWgTargetCtas + tiles - 1) / tiles));
+  sp = std::max(sp, 1ll);
+  p.rows = ((n_rows + sp - 1) / sp + 31) / 32 * 32;
+  p.n_split = (int)((n_rows + p.rows - 1) / p.rows);     // no split is empty
+  return p;
+}
+
+__device__ __forceinline__ float lin_comp(const float4& v, int e) { return e == 0 ? v.x : e == 1 ? v.y : e == 2 ? v.z : v.w; }
+
+template <int O>
+__global__ void __launch_bounds__(kLinThreads, 1)
+k_linear_bwd_weight(const float* __restrict__ dY, long long ldy, const float* __restrict__ A, long long lda,
+                    const float* __restrict__ row_scale, int n_rep, long long N, int n_in, long long rows_per_split,
+                    int col_tiles, float* __restrict__ partial) {
+  using S = WgSmem<O>;
+  constexpr int kTO = S::kTO, kN = S::kN, kSt = S::kSt, kPer = S::kPer;
+  extern __shared__ unsigned char lin_raw[];
+  const unsigned base = (lin_smem_u32(lin_raw) + 1023u) & ~1023u;
+  unsigned char* gbase = lin_raw + (base - lin_smem_u32(lin_raw));
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+  const int col_tile = (int)(blockIdx.x % (unsigned)col_tiles);          // the column tiles of one split run side by side
+  const int o_tile = (int)(blockIdx.x / (unsigned)col_tiles % (O / kTO));  // and share its dY rows through L2
+  const int split = (int)(blockIdx.x / (unsigned)col_tiles / (O / kTO));
+  const long long r_begin = split * rows_per_split, r_end = min(N, r_begin + rows_per_split);
+  const int n_kb = (int)((r_end - r_begin + kLinBK - 1) / kLinBK);
+  const int o0 = o_tile * kTO, c0 = col_tile * S::kTC, n_a = n_in / n_rep;
+  partial += (long long)split * O * n_in;
+
+  // block b of a K block: b < 2 kTO -> dY columns o0 + 4 (b >> 3), else a columns c0 + 4 ((b - 2 kTO) >> 3); rows 4 (b & 7)..+3
+  auto fetch = [&](int kb, float4 (&dst)[kPer][4]) {
+#pragma unroll
+    for (int m = 0; m < kPer; ++m) {
+      const int b = tid + m * kLinThreads;
+      if (b >= S::kBlocks) break;
+      const long long i0 = r_begin + (long long)kb * kLinBK + 4 * (b & 7);
+      const bool is_y = b < 2 * kTO;
+      const int q = (is_y ? b : b - 2 * kTO) >> 3;
+      const int c = is_y ? o0 + 4 * q : c0 + 4 * q;
+      const int sc = is_y ? 0 : c / n_a;                                  // n_a % 32 == 0: one scaler per unit
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const long long i = i0 + r;
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (kb < n_kb && i < r_end) {
+          if (is_y) {
+            v = __ldg(reinterpret_cast<const float4*>(dY + i * ldy + c));
+          } else if (c < n_in) {
+            v = __ldg(reinterpret_cast<const float4*>(A + i * lda + (c - sc * n_a)));
+            if (row_scale) {                                                 // the forward loaders' fl(c_s(i) * a)
+              const float f = __ldg(row_scale + i * n_rep + sc);
+              v.x = __fmul_rn(v.x, f); v.y = __fmul_rn(v.y, f); v.z = __fmul_rn(v.z, f); v.w = __fmul_rn(v.w, f);
+            }
+          }
+        }
+        dst[m][r] = v;
+      }
+    }
+  };
+  // transpose the 4 x 4 block in registers, split, store four K-major units
+  auto stage_store = [&](const float4 (&src)[kPer][4], unsigned char* st) {
+#pragma unroll
+    for (int m = 0; m < kPer; ++m) {
+      const int b = tid + m * kLinThreads;
+      if (b >= S::kBlocks) break;
+      const bool is_y = b < 2 * kTO;
+      const int q = (is_y ? b : b - 2 * kTO) >> 3, jj = b & 7;
+      unsigned char* hi_t = st + (is_y ? 0 : 2 * S::kYTile);
+      unsigned char* lo_t = hi_t + (is_y ? S::kYTile : S::kATile);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        float4 hi, lo;
+        const float v0 = lin_comp(src[m][0], e), v1 = lin_comp(src[m][1], e), v2 = lin_comp(src[m][2], e), v3 = lin_comp(src[m][3], e);
+        hi.x = lin_tf32(v0); lo.x = lin_tf32(v0 - hi.x);
+        hi.y = lin_tf32(v1); lo.y = lin_tf32(v1 - hi.y);
+        hi.z = lin_tf32(v2); lo.z = lin_tf32(v2 - hi.z);
+        hi.w = lin_tf32(v3); lo.w = lin_tf32(v3 - hi.w);
+        const unsigned off = lin_swz(4 * q + e, jj);
+        *reinterpret_cast<float4*>(hi_t + off) = hi;
+        *reinterpret_cast<float4*>(lo_t + off) = lo;
+      }
+    }
+  };
+
+  const unsigned y_off = O == 64 ? 0u : (unsigned)(wg * 64 * 128);           // this warpgroup's 64 dW rows
+  const unsigned a_off = O == 64 ? (unsigned)(wg * 64 * 128) : 0u;           // and its kN columns
+  float acc[kN / 2], corr[kN / 2];
+#pragma unroll
+  for (int i = 0; i < kN / 2; ++i) { acc[i] = 0.f; corr[i] = 0.f; }
+  const int wr = (warp & 3) * 16 + (lane >> 2);
+  const long long o_lo = o0 + (O == 64 ? 0 : wg * 64) + wr;                  // dW rows of registers 4j, 4j + 1 (+8: 4j + 2, 4j + 3)
+  const int c_w = c0 + (O == 64 ? wg * 64 : 0) + 2 * (lane & 3);
+  float* part = reinterpret_cast<float*>(gbase + kSt * S::kStage);          // word i * 256 + tid: thread-private
+  bool first = true;
+  auto fold = [&]() {                                                        // part (+)= acc + corr
+#pragma unroll
+    for (int i = 0; i < kN / 2; ++i) {
+      const float v = acc[i] + corr[i];
+      part[i * kLinThreads + tid] = first ? v : part[i * kLinThreads + tid] + v;
+    }
+    first = false;
+  };
+  float4 pre[kWgAhead][kPer][4];
+#pragma unroll
+  for (int u = 0; u < kWgAhead; ++u) fetch(u, pre[u]);
+  int s = 0;
+  for (int kb0 = 0; kb0 < n_kb; kb0 += kWgAhead) {
+#pragma unroll
+    for (int u = 0; u < kWgAhead; ++u) {
+      const int kb = kb0 + u;
+      if (kb >= n_kb) break;
+      // stage s was last read by the MMAs of step kb - 2: every warp has waited for them (wait_group 1 after step kb - 1)
+      __syncthreads();
+      unsigned char* st = gbase + s * S::kStage;
+      stage_store(pre[u], st);
+      fetch(kb + kWgAhead, pre[u]);
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      __syncthreads();
+      const unsigned sa = base + s * S::kStage;
+      const unsigned y_hi = sa + y_off, y_lo = sa + S::kYTile + y_off;
+      const unsigned a_hi = sa + 2 * S::kYTile + a_off, a_lo = a_hi + S::kATile;
+      lin_fence_acc(acc); lin_fence_acc(corr);
+      asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll
+      for (int ks = 0; ks < kLinBK / 8; ++ks) {
+        const unsigned ko = ks * 32;
+        lin_wgmma<kN>(corr, lin_desc(y_hi + ko), lin_desc(a_lo + ko));
+        lin_wgmma<kN>(corr, lin_desc(y_lo + ko), lin_desc(a_hi + ko));
+        lin_wgmma<kN>(acc, lin_desc(y_hi + ko), lin_desc(a_hi + ko));
+      }
+      asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+      if ((kb + 1) % (kWgFoldRows / kLinBK) == 0 || kb + 1 == n_kb) {
+        asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+        lin_fence_acc(acc); lin_fence_acc(corr);
+        fold();
+#pragma unroll
+        for (int i = 0; i < kN / 2; ++i) { acc[i] = 0.f; corr[i] = 0.f; }
+      } else {
+        asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+        lin_fence_acc(acc); lin_fence_acc(corr);
+      }
+      if (++s == kSt) s = 0;
+    }
+  }
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");   // (the last step folded: nothing is in flight)
+  // the partial tile -> the split's tile of the workspace (or dW), two adjacent columns per store
+#pragma unroll
+  for (int jj = 0; jj < kN / 8; ++jj) {
+    const int c = c_w + jj * 8;
+    if (c >= n_in) continue;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      *reinterpret_cast<float2*>(partial + (o_lo + 8 * h) * n_in + c) =
+          make_float2(part[(4 * jj + 2 * h) * kLinThreads + tid], part[(4 * jj + 2 * h + 1) * kLinThreads + tid]);
+  }
+}
+
+// dW = sum over the splits of their partials, in ascending split order (one float4 per thread)
+__global__ void k_sum_splits(const float* __restrict__ P, int n_split, long long n4, float* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n4) return;
+  const float4* p = reinterpret_cast<const float4*>(P);
+  float4 t = __ldg(p + i);
+  for (int sp = 1; sp < n_split; ++sp) {
+    const float4 v = __ldg(p + sp * n4 + i);
+    t.x = t.x + v.x; t.y = t.y + v.y; t.z = t.z + v.z; t.w = t.w + v.w;
+  }
+  reinterpret_cast<float4*>(out)[i] = t;
+}
+
+template <int O>
+static int launch_bwd_weight(const float* dY, long long ldy, const float* A, long long lda, const float* row_scale, int n_rep,
+                             long long N, int n_in, const BwdWeightPlan& p, float* partial, cudaStream_t st) {
+  auto kern = k_linear_bwd_weight<O>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    PNA_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WgSmem<O>::kBytes));
+    attr_set = true;
+  }
+  const unsigned grid = (unsigned)p.n_split * p.o_tiles * p.col_tiles;
+  kern<<<grid, kLinThreads, WgSmem<O>::kBytes, st>>>(dY, ldy, A, lda, row_scale, n_rep, N, n_in, p.rows, p.col_tiles, partial);
   PNA_CUDA_TRY(cudaGetLastError());
   return PNA_OK;
 }
@@ -365,6 +667,89 @@ extern "C" int pna_linear_scaled_fwd(const float* a, int64_t lda, const float* r
   PNA_REQUIRE(row_scale != nullptr || n_rows == 0, PNA_ERR_BAD_ARG, "pna_linear_scaled_fwd: row_scale is null");
   return linear_common(a, lda, row_scale, n_scalers, weight, bias, y, ldy, n_rows, n_in, n_out, workspace, workspace_bytes, stream,
                        "pna_linear_scaled_fwd");
+}
+
+// ---- backward ----
+static int bwd_check_shape(int64_t n_rows, int32_t n_in, int32_t n_out, int32_t n_rep, const char* who) {
+  PNA_REQUIRE(n_rows >= 0 && n_in > 0 && n_out > 0 && n_rep >= 1 && n_rep <= PNA_MAX_SCALERS, PNA_ERR_BAD_ARG, "%s: bad sizes", who);
+  PNA_REQUIRE(n_in % n_rep == 0 && (n_in / n_rep) % kLinBK == 0, PNA_ERR_UNSUPPORTED,
+              "%s: n_in / n_scalers must be a multiple of %d", who, kLinBK);
+  PNA_REQUIRE(n_out == 64 || n_out == 128 || n_out == 256, PNA_ERR_UNSUPPORTED, "%s: n_out must be 64, 128 or 256", who);
+  return PNA_OK;
+}
+static size_t bwd_data_bytes(int32_t n_in, int32_t n_out, int32_t n_rep) {      // the slabs' weight images
+  const int n_cols = n_in / n_rep, os = bwd_data_slab(n_cols);
+  return 2ull * (size_t)n_out * n_rep * (size_t)((n_cols + os - 1) / os * os) * sizeof(float);
+}
+static size_t bwd_weight_bytes(int64_t n_rows, int32_t n_in, int32_t n_out) {   // the splits' partials (none for one split)
+  const BwdWeightPlan p = bwd_weight_plan(n_rows, n_in, n_out);
+  return p.n_split > 1 ? (size_t)p.n_split * n_out * n_in * sizeof(float) : 0;
+}
+
+extern "C" int pna_linear_bwd_workspace_bytes(int64_t n_rows, int32_t n_in, int32_t n_out, int32_t n_scalers, size_t* bytes) {
+  PNA_REQUIRE(bytes != nullptr, PNA_ERR_BAD_ARG, "pna_linear_bwd_workspace_bytes: bytes is null");
+  const int rc = bwd_check_shape(n_rows, n_in, n_out, n_scalers, "pna_linear_bwd_workspace_bytes");
+  if (rc != PNA_OK) return rc;
+  *bytes = std::max(bwd_data_bytes(n_in, n_out, n_scalers), n_rows > 0 ? bwd_weight_bytes(n_rows, n_in, n_out) : 0);
+  return PNA_OK;
+}
+
+extern "C" int pna_linear_bwd_data(const float* grad_y, int64_t ld_grad_y, const float* row_scale, int32_t n_scalers, const float* weight,
+                                   float* grad_a, int64_t ld_grad_a, int64_t n_rows, int32_t n_in, int32_t n_out, void* workspace,
+                                   size_t workspace_bytes, pna_stream_t stream) {
+  const char* who = "pna_linear_bwd_data";
+  const int rc = bwd_check_shape(n_rows, n_in, n_out, n_scalers, who);
+  if (rc != PNA_OK) return rc;
+  if (n_rows == 0) return PNA_OK;
+  PNA_REQUIRE(grad_y && weight && grad_a && workspace, PNA_ERR_BAD_ARG, "%s: null pointer", who);
+  PNA_REQUIRE(row_scale || n_scalers == 1, PNA_ERR_BAD_ARG, "%s: row_scale is null with %d scalers", who, n_scalers);
+  PNA_REQUIRE(workspace_bytes >= bwd_data_bytes(n_in, n_out, n_scalers), PNA_ERR_WORKSPACE, "%s: workspace too small", who);
+  PNA_REQUIRE(((reinterpret_cast<uintptr_t>(grad_y) | reinterpret_cast<uintptr_t>(grad_a) | reinterpret_cast<uintptr_t>(workspace)) &
+               15u) == 0 && ld_grad_y % 4 == 0 && ld_grad_a % 4 == 0,
+              PNA_ERR_UNSUPPORTED, "%s: grad_y, grad_a, workspace must be 16-byte aligned with pitches that are multiples of 4", who);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int n_cols = n_in / n_scalers, os = bwd_data_slab(n_cols), n_slabs = (n_cols + os - 1) / os;
+  float* img = static_cast<float*>(workspace);
+  const long long units = (long long)n_slabs * (n_out * n_scalers / kLinBK) * 8 * os;
+  k_split_weight_t<<<(unsigned)((units + 255) / 256), 256, 0, st>>>(weight, n_out, n_in, n_scalers, os, n_slabs, img);
+  PNA_CUDA_TRY(cudaGetLastError());
+  // a chain of at most kLinFoldSteps K blocks is never folded: the non-folding instance, whose wgmmas ptxas does not serialize
+  const bool fold = n_out * n_scalers / kLinBK > kLinFoldSteps;
+  if (os == 64)
+    return fold ? launch_linear<64, true>(grad_y, ld_grad_y, row_scale, n_scalers, img, nullptr, grad_a, ld_grad_a, n_rows, n_out, st, n_slabs, n_cols)
+                : launch_linear<64>(grad_y, ld_grad_y, row_scale, n_scalers, img, nullptr, grad_a, ld_grad_a, n_rows, n_out, st, n_slabs, n_cols);
+  return fold ? launch_linear<128, true>(grad_y, ld_grad_y, row_scale, n_scalers, img, nullptr, grad_a, ld_grad_a, n_rows, n_out, st, n_slabs, n_cols)
+              : launch_linear<128>(grad_y, ld_grad_y, row_scale, n_scalers, img, nullptr, grad_a, ld_grad_a, n_rows, n_out, st, n_slabs, n_cols);
+}
+
+extern "C" int pna_linear_bwd_weight(const float* grad_y, int64_t ld_grad_y, const float* a, int64_t lda, const float* row_scale,
+                                     int32_t n_scalers, float* grad_weight, int64_t n_rows, int32_t n_in, int32_t n_out, void* workspace,
+                                     size_t workspace_bytes, pna_stream_t stream) {
+  const char* who = "pna_linear_bwd_weight";
+  const int rc = bwd_check_shape(n_rows, n_in, n_out, n_scalers, who);
+  if (rc != PNA_OK) return rc;
+  if (n_rows == 0) return PNA_OK;
+  PNA_REQUIRE(grad_y && a && grad_weight, PNA_ERR_BAD_ARG, "%s: null pointer", who);
+  PNA_REQUIRE(row_scale || n_scalers == 1, PNA_ERR_BAD_ARG, "%s: row_scale is null with %d scalers", who, n_scalers);
+  const size_t need = bwd_weight_bytes(n_rows, n_in, n_out);
+  PNA_REQUIRE(workspace_bytes >= need && (workspace || need == 0), PNA_ERR_WORKSPACE, "%s: workspace too small", who);
+  PNA_REQUIRE(((reinterpret_cast<uintptr_t>(grad_y) | reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(grad_weight) |
+                reinterpret_cast<uintptr_t>(workspace)) & 15u) == 0 && ld_grad_y % 4 == 0 && lda % 4 == 0,
+              PNA_ERR_UNSUPPORTED, "%s: grad_y, a, grad_weight, workspace must be 16-byte aligned with pitches that are multiples of 4", who);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const BwdWeightPlan p = bwd_weight_plan(n_rows, n_in, n_out);
+  float* partial = p.n_split > 1 ? static_cast<float*>(workspace) : grad_weight;
+  int r;
+  switch (n_out) {
+    case 64: r = launch_bwd_weight<64>(grad_y, ld_grad_y, a, lda, row_scale, n_scalers, n_rows, n_in, p, partial, st); break;
+    case 128: r = launch_bwd_weight<128>(grad_y, ld_grad_y, a, lda, row_scale, n_scalers, n_rows, n_in, p, partial, st); break;
+    default: r = launch_bwd_weight<256>(grad_y, ld_grad_y, a, lda, row_scale, n_scalers, n_rows, n_in, p, partial, st); break;
+  }
+  if (r != PNA_OK || p.n_split == 1) return r;
+  const long long n4 = (long long)n_out * n_in / 4;
+  k_sum_splits<<<(unsigned)((n4 + 255) / 256), 256, 0, st>>>(partial, p.n_split, n4, grad_weight);
+  PNA_CUDA_TRY(cudaGetLastError());
+  return PNA_OK;
 }
 
 namespace pna {

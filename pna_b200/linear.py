@@ -8,9 +8,15 @@ the kernel is an accelerator for one GEMM shape family, not a requirement of the
 ``a`` is the ``[N, A*F]`` result of the identity scaler alone and the S scaled copies the reference concatenates
 (pna.py:247-249) are regenerated in registers by the kernel's loaders -- ``linear(cat_s(row_scale[:, s:s+1] * a), W, b)``
 without the ``[N, S*A*F]`` tensor ever being written or read.
+
+Backward: the input gradient runs on the tensor cores (``pna_linear_bwd_data``, same accuracy, no atomics; the compact one
+never forms the scaled copies).  The weight gradient stays a library fp32 GEMM (``library_grad_weight``): at config 2 on
+H100 cuBLAS is faster than the tensor-core ``pna_linear_bwd_weight`` (DESIGN section 5), which ``linear_bwd_tf32x3``
+still exposes.
 """
 from __future__ import annotations
 
+import ctypes as C
 import os
 from typing import Optional
 
@@ -45,6 +51,50 @@ def linear_tf32x3(a: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Te
     return y
 
 
+def linear_bwd_tf32x3(gy: torch.Tensor, a: torch.Tensor, row_scale: Optional[torch.Tensor], weight: torch.Tensor,
+                      need_a: bool = True, need_w: bool = True):
+    """(grad a, grad weight) of ``linear_tf32x3`` (row_scale None) or ``linear_scaled_tf32x3`` through the C ABI (no
+    autograd); a gradient that is not needed is not computed and comes back as None."""
+    if not (need_a or need_w):
+        return None, None
+    n, ka = a.shape
+    o, k = weight.shape
+    s = 1 if row_scale is None else row_scale.size(1)
+    dev = a.device
+    if not gy.is_contiguous() or gy.data_ptr() % 16:
+        gy = gy.clone(memory_format=torch.contiguous_format)
+    w = weight.detach().contiguous()
+    rs = None if row_scale is None else row_scale.data_ptr()
+    ga = torch.empty((n, ka), dtype=torch.float32, device=dev) if need_a else None
+    gw = torch.empty((o, k), dtype=torch.float32, device=dev) if need_w else None
+    L = _lib.lib()
+    nb = C.c_size_t(0)
+    _lib.check(L.pna_linear_bwd_workspace_bytes(n, k, o, s, C.byref(nb)))
+    ws = torch.empty((nb.value + 3) // 4, dtype=torch.float32, device=dev)        # one buffer for both calls (stream order)
+    with torch.cuda.device(dev):
+        st = torch.cuda.current_stream(dev).cuda_stream
+        if ga is not None:
+            _lib.check(L.pna_linear_bwd_data(gy.data_ptr(), gy.stride(0), rs, s, w.data_ptr(), ga.data_ptr(), ga.stride(0), n, k, o,
+                                             ws.data_ptr(), nb.value, st))
+        if gw is not None:
+            _lib.check(L.pna_linear_bwd_weight(gy.data_ptr(), gy.stride(0), a.data_ptr(), a.stride(0), rs, s, gw.data_ptr(), n, k, o,
+                                               ws.data_ptr(), nb.value, st))
+    return ga, gw
+
+
+def library_grad_weight(gy: torch.Tensor, a: torch.Tensor, row_scale: Optional[torch.Tensor], weight: torch.Tensor) -> torch.Tensor:
+    """grad weight of ``linear_tf32x3`` / ``linear_scaled_tf32x3`` as library fp32 GEMMs (cuBLAS: deterministic with a fixed
+    workspace, as torch.use_deterministic_algorithms requires); with row scales one scaler block at a time, each
+    ``fl(c_s * a)`` a temporary of a's size."""
+    if row_scale is None:
+        return gy.t() @ a
+    ka = a.size(1)
+    gw = torch.empty_like(weight)
+    for s in range(row_scale.size(1)):
+        torch.mm(gy.t(), a * row_scale[:, s:s + 1], out=gw[:, s * ka:(s + 1) * ka])
+    return gw
+
+
 class _Linear3xTF32(torch.autograd.Function):
     @staticmethod
     def forward(ctx, a, weight, bias):
@@ -55,8 +105,8 @@ class _Linear3xTF32(torch.autograd.Function):
     @staticmethod
     def backward(ctx, gy):
         a, weight = ctx.saved_tensors
-        ga = gy @ weight if ctx.needs_input_grad[0] else None
-        gw = gy.t() @ a if ctx.needs_input_grad[1] else None
+        ga, _ = linear_bwd_tf32x3(gy, a, None, weight, ctx.needs_input_grad[0], False)
+        gw = library_grad_weight(gy, a, None, weight) if ctx.needs_input_grad[1] else None
         gb = gy.sum(0) if (ctx.has_bias and ctx.needs_input_grad[2]) else None
         return ga, gw, gb
 
@@ -105,7 +155,7 @@ def linear_scaled_tf32x3(a: torch.Tensor, row_scale: torch.Tensor, weight: torch
 
 
 class _LinearScaled3xTF32(torch.autograd.Function):
-    """Backward in library GEMMs, one scaler block at a time (the scaled copies are temporaries of [N, A*F])."""
+    """The scale factors are constants of the graph: no gradient for row_scale."""
 
     @staticmethod
     def forward(ctx, a, row_scale, weight, bias):
@@ -116,15 +166,8 @@ class _LinearScaled3xTF32(torch.autograd.Function):
     @staticmethod
     def backward(ctx, gy):
         a, row_scale, weight = ctx.saved_tensors
-        ka = a.size(1)
-        ga = torch.zeros_like(a) if ctx.needs_input_grad[0] else None
-        gw = torch.empty_like(weight) if ctx.needs_input_grad[2] else None
-        for s in range(row_scale.size(1)):
-            c = row_scale[:, s:s + 1]
-            if ga is not None:
-                ga.addcmul_(gy @ weight[:, s * ka:(s + 1) * ka], c)
-            if gw is not None:
-                torch.mm(gy.t(), a * c, out=gw[:, s * ka:(s + 1) * ka])
+        ga, _ = linear_bwd_tf32x3(gy, a, row_scale, weight, ctx.needs_input_grad[0], False)
+        gw = library_grad_weight(gy, a, row_scale, weight) if ctx.needs_input_grad[2] else None
         gb = gy.sum(0) if (ctx.has_bias and ctx.needs_input_grad[3]) else None
         return ga, None, gw, gb
 
