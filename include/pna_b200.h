@@ -47,6 +47,12 @@ enum pna_dtype { PNA_F32 = 0, PNA_BF16 = 1 };
 /* Aggregator codes (order of appearance in the layer's ctor list fixes the column layout,
  * pna.py:70,153-154).  Packed 4 bits each, first aggregator in the low nibble. */
 enum pna_aggr { PNA_AGGR_SUM = 0, PNA_AGGR_MEAN = 1, PNA_AGGR_MIN = 2, PNA_AGGR_MAX = 3, PNA_AGGR_VAR = 4, PNA_AGGR_STD = 5,
+                /* central moments of order 3, 4, 5 (models/pytorch/pna/aggregators.py:122-146):
+                     mu = sum / d,  M_k = (sum over slots of (m - mu)^k) / d,  r_k = sign(M_k) (|M_k| + 1e-5)^(1/k),  d == 0: 0.
+                   Taken by pna_aggregate_fwd, pna_aggregate_bwd and pna_aggregate_bwd_slots; pna_aggregate_bwd_coef and
+                   descriptors with peer_gathered or row_ids return PNA_ERR_UNSUPPORTED for them.  Rows at/above the split
+                   threshold are merged in fixed chunk order (no atomics).  Rounding order: pna_b200/csrc/pna_aggregate_moments.cuh */
+                PNA_AGGR_MOMENT3 = 6, PNA_AGGR_MOMENT4 = 7, PNA_AGGR_MOMENT5 = 8,
                 PNA_AGGR_SKIP = 15 /* keep the column slot but do not write it: lets two calls with different edge
                                        sets / messages fill one output row (dense reference layer, where max/min and
                                        mean/std see different messages: models/pytorch/pna/aggregators.py:30-51) */ };

@@ -17,7 +17,8 @@ LIB_PATH = os.environ.get("PNA_B200_LIB") or os.path.join(_HERE, "libpna_sm90.so
 CUDA_SOURCES = [os.path.join(_HERE, "csrc", n) for n in
                 ("pna_aggregate.cu", "pna_aggregate_f32_vec.cu", "pna_aggregate_f32_scalar.cu", "pna_aggregate_bf16_vec.cu",
                  "pna_aggregate_bf16_scalar.cu", "pna_aggregate_f32_fsplit.cu", "pna_aggregate_bwd.cu", "pna_linear.cu", "pna_csr.cu", "pna_peer.cu", "pna_misc.cu")]
-CUDA_HEADERS = [os.path.join(_HERE, "csrc", n) for n in ("common.cuh", "pna_aggregate.cuh", "pna_aggregate_impl.cuh")] + [
+CUDA_HEADERS = [os.path.join(_HERE, "csrc", n) for n in ("common.cuh", "pna_aggregate.cuh", "pna_aggregate_impl.cuh",
+                                                                   "pna_aggregate_moments.cuh")] + [
     os.path.join(REPO_ROOT, "include", "pna_b200.h")]
 BUILD_DIR = os.path.join(_HERE, "csrc", "build")
 
@@ -31,6 +32,10 @@ ABI_VERSION = 8
 PNA_OK = 0
 PNA_F32, PNA_BF16 = 0, 1
 AGGR_CODES = {"sum": 0, "mean": 1, "min": 2, "max": 3, "var": 4, "std": 5, "_skip": 15}
+# the central moments of the dense registry (PNA_AGGR_MOMENT3..5): a separate table, merged where the aggregation packs its
+# list, so that AGGR_CODES stays the set every flavour's layers accept
+MOMENTS = ("moment3", "moment4", "moment5")
+ALL_AGGR_CODES = {**AGGR_CODES, "moment3": 6, "moment4": 7, "moment5": 8}
 SCALER_CODES = {"identity": 0, "amplification": 1, "attenuation": 2, "linear": 3, "inverse_linear": 4}
 FLAG_ZERO_ISOLATED, FLAG_SKIP_LIGHT, FLAG_SKIP_HUBS, FLAG_RELU_VAR, FLAG_GATHER_L1 = 1, 2, 4, 8, 16
 (QUERY_ABI_VERSION, QUERY_SM_ARCH, QUERY_DEFAULT_SPLIT, QUERY_DEFAULT_CHUNK, QUERY_DEVICE_SM_COUNT,

@@ -101,7 +101,7 @@ def aggregate_forward(gathered: torch.Tensor, csr: CSRGraph, aggregators: Names,
     if messages_in_csr_order:
         if gathered.size(0) != csr.n_edges:
             raise ValueError("messages_in_csr_order needs one row per CSR slot")
-    n_aggr, aggr_codes = _lib.pack_codes(aggregators, _lib.AGGR_CODES, "aggregator")
+    n_aggr, aggr_codes = _lib.pack_codes(aggregators, _lib.ALL_AGGR_CODES, "aggregator")
     n_scal, scal_codes = _lib.pack_codes(scalers, _lib.SCALER_CODES, "scaler")
     if row_bias is not None:
         row_bias = _rows2d(row_bias.to(gathered.dtype), "row_bias")
@@ -197,7 +197,7 @@ def aggregate_backward(grad_out: torch.Tensor, gathered: torch.Tensor, csr: CSRG
     gathered = _rows2d(gathered, "gathered")
     F = int(gathered.size(1))
     N = csr.n_nodes
-    n_aggr, aggr_codes = _lib.pack_codes(aggregators, _lib.AGGR_CODES, "aggregator")
+    n_aggr, aggr_codes = _lib.pack_codes(aggregators, _lib.ALL_AGGR_CODES, "aggregator")
     n_scal, scal_codes = _lib.pack_codes(scalers, _lib.SCALER_CODES, "scaler")
     grad_out = _rows2d(grad_out.to(gathered.dtype), "grad_out")
     if row_bias is not None:
@@ -230,8 +230,9 @@ def aggregate_backward(grad_out: torch.Tensor, gathered: torch.Tensor, csr: CSRG
     if deterministic:
         _backward_deterministic(d, grad_out, ld_go, gathered, csr, gg, gb, messages_in_csr_order)
         return gg, gb
+    # moments have no coefficient form (their per-slot gradient is a polynomial of degree k-1 in m): atomic path
     if messages_in_csr_order or csr.n_edges == 0 or csr.sources_unique or backward_mode() == "atomic" \
-            or 2 * _round_up(F, 4) > _lib.query(_lib.QUERY_MAX_FEATURES):
+            or any(a in _lib.MOMENTS for a in _names(aggregators)) or 2 * _round_up(F, 4) > _lib.query(_lib.QUERY_MAX_FEATURES):
         with torch.cuda.device(dev):
             _lib.check(_lib.lib().pna_aggregate_bwd(C.byref(d), grad_out.data_ptr(), ld_go, gg.data_ptr(), F, _ptr(gb), F,
                                                     torch.cuda.current_stream(dev).cuda_stream))
@@ -301,7 +302,8 @@ def backward_mode() -> str:
     feature chunk; ``PNA_B200_BWD=coef`` = per-destination coefficient rows (``pna_aggregate_bwd_coef``), their sums over the
     transposed graph through the forward kernels, ``pna_aggregate_bwd_combine`` -- atomics only for min / max.  The
     coefficient path avoids the atomics that contend on hot source rows (power-law graphs), but regrouping sum_i (c0_i + c1_i x_j) into sum_i c0_i + x_j sum_i c1_i cancels badly where many rows have var ~ 0
-    (2.6x the fp32 error of the per-edge evaluation on a power-law multigraph), so it stays opt-in.
+    (2.6x the fp32 error of the per-edge evaluation on a power-law multigraph), so it stays opt-in.  Calls whose list contains a
+    moment aggregator take the atomic path under ``PNA_B200_BWD=coef``: a moment's gradient is not c0 + c1 * m.
     Under ``torch.use_deterministic_algorithms(True)`` (``warn_only`` too) "deterministic", whatever PNA_B200_BWD says: per-slot
     gradients (``pna_aggregate_bwd_slots``) summed over the reversed edges by the forward kernel, no floating-point atomics,
     the same bits on every run."""

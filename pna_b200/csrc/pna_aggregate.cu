@@ -8,6 +8,31 @@ int launch_typed(const KParams& p, cudaStream_t st);   // defined in pna_aggrega
 
 static bool aligned16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15u) == 0; }
 
+// The moment columns (pna_aggregate_moments.cuh), after the existing kernels have written every other column.
+template <typename T>
+static int launch_moments_fwd(const MParams& p, cudaStream_t st) {
+  const unsigned gy = (unsigned)((p.F + 31) / 32);
+  constexpr long long per_block = kMomThreads / 32;
+  if (!(p.flags & PNA_FLAG_SKIP_LIGHT)) {
+    const long long gx = (p.n_rows + per_block - 1) / per_block;
+    PNA_REQUIRE(gx <= 0x7fffffffll, PNA_ERR_UNSUPPORTED, "pna_aggregate_fwd: too many rows");
+    k_mom_rows<T><<<dim3((unsigned)gx, gy), kMomThreads, 0, st>>>(p);
+    PNA_CUDA_TRY(cudaGetLastError());
+  }
+  if (!(p.flags & PNA_FLAG_SKIP_HUBS) && p.n_hubs > 0) {
+    const unsigned gc = (unsigned)((p.n_chunks + per_block - 1) / per_block), gh = (unsigned)((p.n_hubs + per_block - 1) / per_block);
+    k_mom_chunk_sum<T, 4><<<dim3(gc, gy), kMomThreads, 0, st>>>(p);
+    PNA_CUDA_TRY(cudaGetLastError());
+    k_mom_hub_mean<4><<<dim3(gh, gy), kMomThreads, 0, st>>>(p);
+    PNA_CUDA_TRY(cudaGetLastError());
+    k_mom_chunk_central<T, 4><<<dim3(gc, gy), kMomThreads, 0, st>>>(p);
+    PNA_CUDA_TRY(cudaGetLastError());
+    k_mom_hub_final<T><<<dim3(gh, gy), kMomThreads, 0, st>>>(p);
+    PNA_CUDA_TRY(cudaGetLastError());
+  }
+  return PNA_OK;
+}
+
 }  // namespace pna
 
 using namespace pna;
@@ -24,8 +49,11 @@ extern "C" int pna_aggregate_fwd(const pna_agg_t* d, pna_stream_t stream) {
   PNA_REQUIRE(d->n_aggr >= 1 && d->n_aggr <= PNA_MAX_AGGR && d->n_scalers >= 1 && d->n_scalers <= PNA_MAX_SCALERS,
               PNA_ERR_BAD_ARG, "pna_aggregate_fwd: n_aggr=%d n_scalers=%d out of range", d->n_aggr, d->n_scalers);
   for (int a = 0; a < d->n_aggr; ++a)
-    PNA_REQUIRE(((d->aggr_codes >> (4 * a)) & 15u) <= PNA_AGGR_STD || ((d->aggr_codes >> (4 * a)) & 15u) == PNA_AGGR_SKIP,
+    PNA_REQUIRE(((d->aggr_codes >> (4 * a)) & 15u) <= PNA_AGGR_MOMENT5 || ((d->aggr_codes >> (4 * a)) & 15u) == PNA_AGGR_SKIP,
                 PNA_ERR_BAD_ARG, "pna_aggregate_fwd: bad aggregator code");
+  const bool moments = moment_orders(d->aggr_codes, d->n_aggr) != 0;
+  PNA_REQUIRE(!moments || (!d->peer_gathered && !d->row_ids), PNA_ERR_UNSUPPORTED,
+              "pna_aggregate_fwd: moment aggregators are not available with peer_gathered or row_ids");
   for (int s = 0; s < d->n_scalers; ++s)
     PNA_REQUIRE(((d->scaler_codes >> (4 * s)) & 15u) <= PNA_SCALE_INVERSE_LINEAR, PNA_ERR_BAD_ARG,
                 "pna_aggregate_fwd: bad scaler code");
@@ -46,7 +74,8 @@ extern "C" int pna_aggregate_fwd(const pna_agg_t* d, pna_stream_t stream) {
   p.n_rows = d->n_rows;
   p.F = d->n_feat; p.T = d->n_towers; p.Ft = d->n_feat / d->n_towers;
   p.has_self = d->self_feat ? 1 : 0;
-  p.nA = d->n_aggr; p.nS = d->n_scalers; p.acodes = d->aggr_codes; p.scodes = d->scaler_codes;
+  p.nA = d->n_aggr; p.nS = d->n_scalers; p.scodes = d->scaler_codes;
+  p.acodes = moments ? strip_moments(d->aggr_codes, d->n_aggr) : d->aggr_codes;   // the moment kernels write those columns
   p.Wt = (p.has_self + p.nA * p.nS) * p.Ft;
   p.avg_log = d->avg_log; p.avg_lin = d->avg_lin;
   p.flags = d->flags; p.split = d->split_threshold; p.chunk = d->chunk_edges;
@@ -83,9 +112,13 @@ extern "C" int pna_aggregate_fwd(const pna_agg_t* d, pna_stream_t stream) {
   bool vec_ok = (p.Ft % vec == 0) && aligned16(p.x) && aligned16(p.out) && (p.ldx % vec == 0) && (p.ldo % vec == 0);
   if (p.bias) vec_ok = vec_ok && aligned16(p.bias) && (p.ldb % vec == 0);
   if (p.self) vec_ok = vec_ok && aligned16(p.self) && (p.lds % vec == 0) && (p.self_tstride % vec == 0);
+  int rc;
   if (d->dtype == PNA_F32) {
-    return vec_ok ? launch_typed<float, 4>(p, st) : launch_typed<float, 1>(p, st);
+    rc = vec_ok ? launch_typed<float, 4>(p, st) : launch_typed<float, 1>(p, st);
   } else {
-    return vec_ok ? launch_typed<__nv_bfloat16, 8>(p, st) : launch_typed<__nv_bfloat16, 1>(p, st);
+    rc = vec_ok ? launch_typed<__nv_bfloat16, 8>(p, st) : launch_typed<__nv_bfloat16, 1>(p, st);
   }
+  if (rc != PNA_OK || !moments) return rc;
+  const MParams mp = moment_params(d);
+  return d->dtype == PNA_F32 ? launch_moments_fwd<float>(mp, st) : launch_moments_fwd<__nv_bfloat16>(mp, st);
 }

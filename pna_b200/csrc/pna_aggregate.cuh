@@ -387,3 +387,5 @@ __device__ __forceinline__ void finalize_row_ds(const KParams& p, const FeatMap<
 }
 
 }  // namespace pna
+
+#include "pna_aggregate_moments.cuh"

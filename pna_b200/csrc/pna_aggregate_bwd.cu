@@ -555,6 +555,35 @@ static int launch_bwd_typed(const BParams& b, cudaStream_t st) {
 
 static bool al16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15u) == 0; }
 
+// The moment term of every slot's gradient (pna_aggregate_moments.cuh), added after the existing kernels have written it.
+template <typename T, bool SLOTS>
+static int launch_moments_bwd(const MParams& p, cudaStream_t st) {
+  const unsigned gy = (unsigned)((p.f1 - p.f0 + 31) / 32);
+  constexpr long long per_block = kMomThreads / 32;
+  const long long gx = (p.n_rows + per_block - 1) / per_block;
+  PNA_REQUIRE(gx <= 0x7fffffffll, PNA_ERR_UNSUPPORTED, "pna_aggregate_bwd: too many rows");
+  k_mom_bwd_rows<T, SLOTS><<<dim3((unsigned)gx, gy), kMomThreads, 0, st>>>(p);
+  PNA_CUDA_TRY(cudaGetLastError());
+  if (p.n_hubs > 0) {
+    const unsigned gc = (unsigned)((p.n_chunks + per_block - 1) / per_block), gh = (unsigned)((p.n_hubs + per_block - 1) / per_block);
+    k_mom_chunk_sum<T, 6><<<dim3(gc, gy), kMomThreads, 0, st>>>(p);
+    PNA_CUDA_TRY(cudaGetLastError());
+    k_mom_hub_mean<6><<<dim3(gh, gy), kMomThreads, 0, st>>>(p);
+    PNA_CUDA_TRY(cudaGetLastError());
+    k_mom_chunk_central<T, 6><<<dim3(gc, gy), kMomThreads, 0, st>>>(p);
+    PNA_CUDA_TRY(cudaGetLastError());
+    k_mom_bwd_hub_coef<T><<<dim3(gh, gy), kMomThreads, 0, st>>>(p);
+    PNA_CUDA_TRY(cudaGetLastError());
+    k_mom_bwd_chunk_grad<T, SLOTS><<<dim3(gc, gy), kMomThreads, 0, st>>>(p);
+    PNA_CUDA_TRY(cudaGetLastError());
+    if (p.gb) {
+      k_mom_bwd_hub_bias<6><<<dim3(gh, gy), kMomThreads, 0, st>>>(p);
+      PNA_CUDA_TRY(cudaGetLastError());
+    }
+  }
+  return PNA_OK;
+}
+
 // ---- phase 3 of the coefficient path: grad_gathered[j] += S0[j] + gathered[j] * S1[j] ------------------------------------
 // sums[j] = [S0 | S1] (S1 at column c1): the 'sum' of the coefficient rows over the out-edges of source row j.
 template <typename T>
@@ -595,6 +624,12 @@ static int bwd_entry(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_o
                 PNA_ERR_BAD_ARG, "pna_aggregate_bwd_slots: bad feature slab [%d, +%d) of %d features", f_begin, f_count, d->n_feat);
     PNA_REQUIRE(ld_grad_slots >= f_count, PNA_ERR_BAD_ARG, "pna_aggregate_bwd_slots: ld_grad_slots < f_count");
   }
+  const bool moments = moment_orders(d->aggr_codes, d->n_aggr) != 0;
+  // a moment's per-slot gradient is a polynomial of degree k-1 in m, not the c0 + c1 * m the coefficient rows regroup
+  PNA_REQUIRE(!moments || !coef, PNA_ERR_UNSUPPORTED,
+              "pna_aggregate_bwd_coef: moment aggregators have no coefficient form; use pna_aggregate_bwd or pna_aggregate_bwd_slots");
+  PNA_REQUIRE(!moments || (!d->peer_gathered && !d->row_ids), PNA_ERR_UNSUPPORTED,
+              "pna_aggregate_bwd: moment aggregators are not available with peer_gathered or row_ids");
   if (d->n_rows == 0) return PNA_OK;
   PNA_REQUIRE(d->gathered && d->rowptr && grad_out && (slots || grad_gathered), PNA_ERR_BAD_ARG, "pna_aggregate_bwd: null pointer");
   PNA_REQUIRE(d->peer_gathered == nullptr, PNA_ERR_UNSUPPORTED, "pna_aggregate_bwd: peer-memory graphs are forward-only");
@@ -613,7 +648,8 @@ static int bwd_entry(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_o
   p.n_rows = d->n_rows;
   p.F = d->n_feat; p.T = d->n_towers; p.Ft = d->n_feat / d->n_towers;
   p.has_self = d->self_feat ? 1 : 0;
-  p.nA = d->n_aggr; p.nS = d->n_scalers; p.acodes = d->aggr_codes; p.scodes = d->scaler_codes;
+  p.nA = d->n_aggr; p.nS = d->n_scalers; p.scodes = d->scaler_codes;
+  p.acodes = moments ? strip_moments(d->aggr_codes, d->n_aggr) : d->aggr_codes;   // the moment kernels add their term
   p.Wt = (p.has_self + p.nA * p.nS) * p.Ft;
   p.avg_log = d->avg_log; p.avg_lin = d->avg_lin;
   p.flags = d->flags; p.split = d->split_threshold; p.chunk = d->chunk_edges;
@@ -643,12 +679,26 @@ static int bwd_entry(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_o
   const int vec = 16 / esz;
   bool vec_ok = (p.Ft % vec == 0) && al16(p.x) && al16(grad_out) && (p.ldx % vec == 0) && (b.ldgo % vec == 0);
   if (p.bias) vec_ok = vec_ok && al16(p.bias) && (p.ldb % vec == 0);
+  const bool f32 = d->dtype == PNA_F32;
+  int rc;
   if (slots) {
-    if (d->dtype == PNA_F32) return vec_ok ? launch_bwd_typed<float, 4, true>(b, st) : launch_bwd_typed<float, 1, true>(b, st);
-    return vec_ok ? launch_bwd_typed<__nv_bfloat16, 8, true>(b, st) : launch_bwd_typed<__nv_bfloat16, 1, true>(b, st);
+    if (f32) rc = vec_ok ? launch_bwd_typed<float, 4, true>(b, st) : launch_bwd_typed<float, 1, true>(b, st);
+    else rc = vec_ok ? launch_bwd_typed<__nv_bfloat16, 8, true>(b, st) : launch_bwd_typed<__nv_bfloat16, 1, true>(b, st);
+  } else {
+    if (f32) rc = vec_ok ? launch_bwd_typed<float, 4, false>(b, st) : launch_bwd_typed<float, 1, false>(b, st);
+    else rc = vec_ok ? launch_bwd_typed<__nv_bfloat16, 8, false>(b, st) : launch_bwd_typed<__nv_bfloat16, 1, false>(b, st);
   }
-  if (d->dtype == PNA_F32) return vec_ok ? launch_bwd_typed<float, 4, false>(b, st) : launch_bwd_typed<float, 1, false>(b, st);
-  return vec_ok ? launch_bwd_typed<__nv_bfloat16, 8, false>(b, st) : launch_bwd_typed<__nv_bfloat16, 1, false>(b, st);
+  if (rc != PNA_OK || !moments) return rc;
+  MParams mp = moment_params(d);
+  mp.go = grad_out; mp.ldgo = ld_grad_out;
+  mp.gb = grad_row_bias; mp.ldgb = ld_grad_row_bias;
+  if (slots) {
+    mp.gs = grad_slots; mp.ldgs = ld_grad_slots;
+    mp.f0 = f_begin; mp.f1 = f_begin + f_count;
+    return f32 ? launch_moments_bwd<float, true>(mp, st) : launch_moments_bwd<__nv_bfloat16, true>(mp, st);
+  }
+  mp.gg = grad_gathered; mp.ldgg = ld_grad_gathered;
+  return f32 ? launch_moments_bwd<float, false>(mp, st) : launch_moments_bwd<__nv_bfloat16, false>(mp, st);
 }
 
 extern "C" int pna_aggregate_bwd(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_out, float* grad_gathered,

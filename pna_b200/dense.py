@@ -14,7 +14,12 @@ Two kernel calls fill one output row (PNA_AGGR_SKIP keeps the other call's colum
 ``self_loop=True`` aggregates over adj + I while the scalers keep the loop-free row degree (``pna_agg_t.scaler_degree``);
 ``var`` is clamped at 0 as the reference does (PNA_FLAG_RELU_VAR).
 Restrictions (documented, not silent): 0/1 adjacency (the reference's weighted sums are not reproduced), aggregators
-mean/max/min/std/sum/var, and -- unlike the reference, which divides by zero -- isolated nodes get PyG semantics.
+mean/max/min/std/sum/var/moment3/moment4/moment5, and -- unlike the reference, which divides by zero -- isolated nodes get
+PyG semantics (a moment of a row without neighbours is 0).
+The moments reduce over dim 2 like mean/std (self first).  ``self_loop=True`` with a moment raises NotImplementedError:
+the reference's ``aggregate_moment`` adds I to adj and then calls ``aggregate_mean(..., self_loop=True)``, which adds I
+again, so its moments are centred on a mean that counts the self loop twice -- not a central moment of any edge set the
+kernel can be given.
 """
 from __future__ import annotations
 
@@ -25,7 +30,8 @@ from .aggregate import aggregate_forward, pna_aggregate
 from .csr import build_csr, tensor_version
 from .nn_blocks import FCLayer, MLP
 
-_SELF_FIRST = ("mean", "std", "sum", "var")
+_SELF_FIRST = ("mean", "std", "sum", "var", "moment3", "moment4", "moment5")
+_MOMENTS = ("moment3", "moment4", "moment5")
 _NBR_FIRST = ("max", "min")
 
 
@@ -85,6 +91,9 @@ class PNALayer(nn.Module):
         for a in self.aggregators:
             if a not in _SELF_FIRST + _NBR_FIRST:
                 raise KeyError(f"aggregator {a!r} is not available on the CUDA path")
+        if self_loop and any(a in _MOMENTS for a in self.aggregators):
+            raise NotImplementedError("dense PNALayer: moment aggregators with self_loop=True are not supported (the reference "
+                                      "centres them on a mean that counts the self loop twice; see the module docstring)")
         self.avg_d = {k: float(v) for k, v in avg_d.items()}
         self.self_loop = self_loop
         self.divide_input = divide_input
