@@ -16,7 +16,7 @@ REPO_ROOT = os.path.dirname(_HERE)
 LIB_PATH = os.environ.get("PNA_B200_LIB") or os.path.join(_HERE, "libpna_sm90.so")   # env override: tuning builds only
 CUDA_SOURCES = [os.path.join(_HERE, "csrc", n) for n in
                 ("pna_aggregate.cu", "pna_aggregate_f32_vec.cu", "pna_aggregate_f32_scalar.cu", "pna_aggregate_bf16_vec.cu",
-                 "pna_aggregate_bf16_scalar.cu", "pna_aggregate_f32_fsplit.cu", "pna_aggregate_bwd.cu", "pna_linear.cu", "pna_csr.cu", "pna_peer.cu", "pna_misc.cu")]
+                 "pna_aggregate_bf16_scalar.cu", "pna_aggregate_bwd.cu", "pna_linear.cu", "pna_csr.cu", "pna_peer.cu", "pna_misc.cu")]
 CUDA_HEADERS = [os.path.join(_HERE, "csrc", n) for n in ("common.cuh", "pna_aggregate.cuh", "pna_aggregate_impl.cuh",
                                                                    "pna_aggregate_moments.cuh")] + [
     os.path.join(REPO_ROOT, "include", "pna_b200.h")]

@@ -47,10 +47,7 @@ def _dynamic_tail(csr: CSRGraph) -> bool:
     """Hand the last 30 % of the row partitions out dynamically (pna_agg_t.work_counter)?  Every grab restarts the warp's
     gather ring (serial latency: counter, partition bounds, first sources, first rows), so it pays only when a
     partition is much more work than that: the config-5 share (420 slots+12*rows per partition) gains, config 2 (49 per
-    partition) loses.  PNA_B200_DYNAMIC_TAIL=0/1 overrides."""
-    env = os.environ.get("PNA_B200_DYNAMIC_TAIL")
-    if env is not None:
-        return env != "0"
+    partition) loses."""
     return csr.n_part > 0 and (csr.n_edges + 12 * csr.n_nodes) / csr.n_part >= DYNAMIC_TAIL_MIN_PARTITION_COST
 
 

@@ -81,24 +81,8 @@ __device__ __forceinline__ DegScales deg_scales(int deg, float avg_log, float av
 // ---- element load/store with fp32 math -------------------------------------------------------------------
 // Gathered rows go through the read-only path (ld.global.nc); the [N, S*A*F] result is written once and never
 // re-read by this library, so it is stored with the streaming (evict-first) policy to keep source rows in L2.
-
-// How the [N, S*A*F] result leaves the SM.  0: st.global.cs (streaming, evict-first) -- the default; 1: plain st.global;
-// 2: st.global.cg; 3: st.global.wt.  A build-time knob for experiments (nvcc -DPNA_STORE_MODE=n).
-#ifndef PNA_STORE_MODE
-#define PNA_STORE_MODE 0
-#endif
 template <typename V>
-__device__ __forceinline__ void store_out(V* p, V v) {
-#if PNA_STORE_MODE == 1
-  *p = v;
-#elif PNA_STORE_MODE == 2
-  __stcg(p, v);
-#elif PNA_STORE_MODE == 3
-  __stwt(p, v);
-#else
-  __stcs(p, v);
-#endif
-}
+__device__ __forceinline__ void store_out(V* p, V v) { __stcs(p, v); }
 
 template <typename T, int VEC>
 struct Io;
@@ -112,15 +96,6 @@ struct Io<float, 4> {
   static __device__ __forceinline__ void store(float* p, const float (&v)[4]) {
     store_out(reinterpret_cast<float4*>(p), make_float4(v[0], v[1], v[2], v[3]));
   }
-};
-
-template <>
-struct Io<float, 2> {
-  typedef float2 Raw;
-  static __device__ __forceinline__ Raw load_raw(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
-  static __device__ __forceinline__ void unpack(const Raw& r, float (&v)[2]) { v[0] = r.x; v[1] = r.y; }
-  static __device__ __forceinline__ void load(const float* p, float (&v)[2]) { unpack(load_raw(p), v); }
-  static __device__ __forceinline__ void store(float* p, const float (&v)[2]) { store_out(reinterpret_cast<float2*>(p), make_float2(v[0], v[1])); }
 };
 
 template <>

@@ -93,7 +93,6 @@ extern "C" int pna_aggregate_fwd(const pna_agg_t* d, pna_stream_t stream) {
                       ? d->n_view_rows : d->n_rows;
   PNA_REQUIRE(p.n_view_rows == d->n_rows || d->n_view_rows == d->n_rows + d->n_chunks, PNA_ERR_BAD_ARG,
               "pna_aggregate_fwd: n_view_rows must be n_rows + n_chunks");
-  p.n_fpass = 0;
   p.work_ctr = d->work_counter; p.n_static = 0;
   p.sdeg = d->scaler_degree;
   // more than 512 chunks in one row: merge the partials with the radix tree (k_hub_tree) before the finalize

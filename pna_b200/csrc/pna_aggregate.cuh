@@ -40,7 +40,6 @@ struct KParams {
   int n_static;            // partitions [0, n_static) are dealt out statically (set by the launcher)
   int hub_merged;          // 1: every split row's total already sits in its first partial slot (k_hub_tree ran)
   const int* sdeg;         // nullable [n_rows]: degree seen by the scalers (default: the in-degree of the row)
-  int n_fpass;             // > 1: the streamed kernel makes this many passes over its rows, one feature block each
   const void* const* peer_x; int peer_shift;   // multi-GPU: x of every rank (NVLink peer pointers), col = owner << shift | row
 };
 

@@ -2,8 +2,6 @@
 // pna_aggregate_{f32,bf16}_{vec,scalar}.cu so the translation units compile in parallel.
 #pragma once
 #include "pna_aggregate.cuh"
-#include <stdlib.h>
-#include <string.h>
 
 namespace pna {
 
@@ -248,73 +246,43 @@ __global__ void __launch_bounds__(kTiledThreads, tiled_min_blocks(VEC, K)) k_row
   }
 }
 
-// ---- rows below the split threshold, TMA-streamed gather (rows of >= 17 128-bit chunks: F >= 68 fp32) ----------
+// ---- rows below the split threshold, streamed gather (rows of >= 17 128-bit chunks: F >= 68 fp32) ---------------
 // Persistent warps: each owns a contiguous range of rows of the LIGHT VIEW (split rows removed, so the in-edges of
 // the range are ONE contiguous stream of slots), the ranges cut at equal-cost boundaries precomputed with the CSR.
-// The warp keeps a double-buffered ring of
-// neighbour feature rows in shared memory: all 32 lanes issue one bulk async copy (cp.async.bulk, the TMA engine's
-// 1-D path, SASS UBLKCP) each -- row x[col[slot]] -> ring slot -- completing on an mbarrier per half; while one half
-// is being reduced (ld.shared.v4, lanes = feature chunks, slot order = CSR order) the other half is in flight.
+// The warp keeps a ring of neighbour feature rows in shared memory, cut into segments of H slots: every lane copies
+// its own 16-byte chunk(s) of each row x[col[slot]] into the ring slot with cp.async (LDGSTS, L2 evict-last hint),
+// one cp.async group per segment, and later reads back exactly those bytes (ld.shared.v4, lanes = feature chunks,
+// slot order = CSR order), so completion is tracked per thread and no lane waits for another.  While one segment is
+// being reduced the others are in flight.
 // Gather latency is hidden by bytes in flight in shared memory instead of by registers or by more warps:
 // 24 warps x 8 KB per SM versus 24 warps x 4 x 512 B with register staging.
 constexpr int kStreamThreads = 128;
 
 __device__ __forceinline__ unsigned smem_u32(const void* ptr) { return (unsigned)__cvta_generic_to_shared(ptr); }
-__device__ __forceinline__ void mbar_init(unsigned bar, unsigned count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned bar, unsigned bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned bar, unsigned parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "WAIT_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONE_%=;\n\t"
-      "bra WAIT_%=;\n\t"
-      "DONE_%=:\n\t}" ::"r"(bar), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(unsigned dst, const void* src, unsigned bytes, unsigned bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-               "l"(__cvta_generic_to_global(src)), "r"(bytes), "r"(bar)
-               : "memory");
-}
 
 // 128-bit shared-memory load through a 32-bit shared address (no generic-address conversion in the loop)
 template <typename T, int VEC>
 __device__ __forceinline__ typename Io<T, VEC>::Raw lds_raw(unsigned addr) {
-  static_assert(sizeof(typename Io<T, VEC>::Raw) == 16 || sizeof(typename Io<T, VEC>::Raw) == 8, "stream path moves 128- or 64-bit chunks");
+  static_assert(sizeof(typename Io<T, VEC>::Raw) == 16, "the stream path moves 128-bit chunks");
   typename Io<T, VEC>::Raw r;
   unsigned* w = reinterpret_cast<unsigned*>(&r);
-  if constexpr (sizeof(typename Io<T, VEC>::Raw) == 16) {
-    unsigned a, b, c, d;
-    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(a), "=r"(b), "=r"(c), "=r"(d) : "r"(addr));
-    w[0] = a; w[1] = b; w[2] = c; w[3] = d;
-  } else {
-    unsigned a, b;
-    asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(a), "=r"(b) : "r"(addr));
-    w[0] = a; w[1] = b;
-  }
+  unsigned a, b, c, d;
+  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(a), "=r"(b), "=r"(c), "=r"(d) : "r"(addr));
+  w[0] = a; w[1] = b; w[2] = c; w[3] = d;
   return r;
 }
 
-#ifndef PNA_STREAM_HALF_BYTES
-#define PNA_STREAM_HALF_BYTES 4096   // bytes of neighbour rows per ring segment per warp
-#endif
-#ifndef PNA_STREAM_STAGES
-#define PNA_STREAM_STAGES 2          // ring segments per warp: one being reduced, the others in flight
-#endif
 // DEPTH scales the ring: 1 for local HBM gathers; 2 when remote rows arrive over NVLink (2-3x the latency, and a row
 // at the head of the in-order ring blocks the rows behind it)
 template <typename T, int VEC, int K, int DEPTH = 1>
 struct StreamGeom {
+  static constexpr int kHalfBytes = 4096;   // bytes of neighbour rows per ring segment per warp (DEPTH 1)
+  static constexpr int kStages = 2;         // ring segments per warp: one being reduced, the others in flight
   static constexpr int kBlockBytes = 32 * VEC * K * (int)sizeof(T);            // bytes of one ring slot
-  static constexpr int kHalf = PNA_STREAM_HALF_BYTES * DEPTH;
+  static constexpr int kHalf = kHalfBytes * DEPTH;
   static constexpr int kH = (kHalf / kBlockBytes) < 4 ? 4 : ((kHalf / kBlockBytes) > 32 ? 32 : (kHalf / kBlockBytes));
-  static constexpr int kStages = PNA_STREAM_STAGES;                              // ring segments ("halves") per warp
   static constexpr int kWarpBytes = kStages * kH * kBlockBytes;
-  static constexpr size_t kSmem = 128 + (size_t)(kStreamThreads / 32) * kWarpBytes;
+  static constexpr size_t kSmem = (size_t)(kStreamThreads / 32) * kWarpBytes;
 };
 
 // 16-byte async copy global -> shared (LDGSTS, L2-only caching) with an L2 eviction-priority hint
@@ -331,15 +299,6 @@ __device__ __forceinline__ void cp_async16(unsigned dst, const void* src, unsign
     asm volatile("cp.async.cg.shared.global.L2::cache_hint [%0], [%1], 16, %2;" ::"r"(dst), "l"(__cvta_generic_to_global(src)), "l"(policy)
                  : "memory");
 }
-// 8-byte variant (feature-split passes: 64-bit chunks per lane); .ca is the only qualifier cp.async allows below 16 bytes
-__device__ __forceinline__ void cp_async8(unsigned dst, const void* src, unsigned long long policy) {
-  asm volatile("cp.async.ca.shared.global.L2::cache_hint [%0], [%1], 8, %2;" ::"r"(dst), "l"(__cvta_generic_to_global(src)), "l"(policy)
-               : "memory");
-}
-template <int BYTES, bool L1 = false>
-__device__ __forceinline__ void cp_async_chunk(unsigned dst, const void* src, unsigned long long policy) {
-  if constexpr (BYTES == 16) cp_async16<L1>(dst, src, policy); else cp_async8(dst, src, policy);
-}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
@@ -348,10 +307,6 @@ __device__ __forceinline__ unsigned long long l2_policy_evict_last() {
   asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
   return pol;
 }
-
-#ifndef PNA_STREAM_TMA
-#define PNA_STREAM_TMA 0   // 1: per-row cp.async.bulk (UBLKCP) + mbarrier; 0: per-lane 16-byte cp.async (LDGSTS) groups
-#endif
 
 // ---- hubs, pass 2: one CTA per hub merges its partials, then the common epilogue ---------------------------
 // kFinGroups lane groups stride over the hub's chunks (group q takes chunks q, q+kFinGroups, ..), each merging in
@@ -470,7 +425,7 @@ __global__ void __launch_bounds__(kStreamThreads, tiled_min_blocks(VEC, K)) k_ro
   constexpr int H = StreamGeom<T, VEC, K, DEPTH>::kH;
   constexpr int SLOT = StreamGeom<T, VEC, K, DEPTH>::kBlockBytes;
   constexpr int NST = StreamGeom<T, VEC, K, DEPTH>::kStages;
-  static_assert(!PNA_STREAM_TMA || NST == 2, "the bulk-copy build variant keeps the two-segment ring");
+  constexpr int CB = 16;               // bytes per lane chunk
   constexpr unsigned FULL = 0xffffffffu;
   constexpr bool PEER = DEPTH > 1;     // the deep-ring instantiations are the ones launched with peer pointers
   extern __shared__ __align__(128) unsigned char smem[];
@@ -479,21 +434,9 @@ __global__ void __launch_bounds__(kStreamThreads, tiled_min_blocks(VEC, K)) k_ro
   const int warp = threadIdx.x >> 5;
   fill_scale_lut(s_scale_lut, p, threadIdx.x, kStreamThreads);
 
-  // shared memory: [warps][2] mbarriers, then per warp a ring of 2*H slots
-  const unsigned smem0 = smem_u32(smem);
-  const unsigned bar0 = smem0 + warp * 16;
-  const unsigned ring = smem0 + 128 + warp * StreamGeom<T, VEC, K, DEPTH>::kWarpBytes;
-#if PNA_STREAM_TMA
-  if (lane == 0) {
-    mbar_init(bar0, 1);
-    mbar_init(bar0 + 8, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncwarp();
-#else
+  // shared memory: per warp a ring of NST*H slots
+  const unsigned ring = smem_u32(smem) + warp * StreamGeom<T, VEC, K, DEPTH>::kWarpBytes;
   const unsigned long long keep = l2_policy_evict_last();   // gathered rows are re-read by other destinations
-  (void)bar0;
-#endif
 
   // this warp's rows: first a contiguous range of the light view cut at equal-cost partition boundaries -- the first
   // n_static partitions are dealt out statically, one contiguous range per warp (one uninterrupted slot stream).  The
@@ -511,38 +454,15 @@ __global__ void __launch_bounds__(kStreamThreads, tiled_min_blocks(VEC, K)) k_ro
   const int Te = __ldg(p.lrowptr + pb) - Q0;      // length of this slot stream
   if (pa < pb) {                                  // warp-uniform; no CTA-wide barrier is used below
   const int* __restrict__ lcol = p.lcol + Q0;
-  // feature passes: with n_fpass > 1 every warp walks its rows n_fpass times, each time over a block of G*VEC*K
-  // features -- the gathered working set of a pass is n_src * (block bytes), sized to stay L2-resident
-  constexpr int CB = VEC * (int)sizeof(T);          // bytes per lane chunk (16, or 8 on the feature-split path)
-  const int n_fpass = p.n_fpass > 1 ? p.n_fpass : 1;
-#pragma unroll 1
- for (int fpass = 0; fpass < n_fpass; ++fpass) {
-  const int fblock = (blockIdx.y * n_fpass + fpass) * (G * VEC * K);
-  const unsigned copy_bytes = (unsigned)(min(G * VEC * K, p.F - fblock) * (int)sizeof(T));
-  (void)copy_bytes;
+  const int fblock = blockIdx.y * (G * VEC * K);
   FeatMap<VEC, G, K> fm;
   fm.init(p, lane, fblock);
 
   // source row of stream position q for this lane.  Past the end of the stream (and for lanes >= H) it is row 0: the
   // ring slot is filled with a row nobody reads, which keeps every copy unconditional -- no per-slot branch
-#if PNA_STREAM_TMA
-  auto source_of = [&](int q) -> int { return (lane < H && q < Te) ? __ldg(lcol + q) : -1; };
-#else
   auto source_of = [&](int q) -> int { return (lane < H && q < Te) ? __ldg(lcol + q) : 0; };
-#endif
-  // issue the copies of half n (positions n*H .. n*H+H-1) whose sources were fetched one step earlier
-#if PNA_STREAM_TMA
-  int tma_issued = 0;
-  auto issue_half = [&](int stage, int src) {
-    const int nvalid = min(H, Te - tma_issued * H);
-    ++tma_issued;
-    const unsigned bar = bar0 + stage * 8;
-    if (lane == 0) mbar_expect_tx(bar, (unsigned)nvalid * copy_bytes);
-    if (src >= 0) bulk_g2s(ring + (stage * H + lane) * SLOT, gathered_row<T>(p, src) + fblock, copy_bytes, bar);
-  };
-#else
-  // every lane copies ITS OWN 16-byte chunk(s) of each neighbour row, and later reads exactly those bytes back:
-  // completion is tracked per thread by cp.async groups, no cross-lane synchronisation is needed at all
+  // issue the copies of segment n (positions n*H .. n*H+H-1) whose sources were fetched one step earlier; each lane
+  // copies only its own chunks (see above)
   const int lane_elems = fblock + lane * VEC;   // this lane's first 16-byte chunk inside a gathered row
   // byte address of this lane's chunk in row 0; a row is one unsigned 32 x 32 -> 64-bit multiply-add away (IMAD.WIDE.U32)
   const char* const xlane = reinterpret_cast<const char*>(static_cast<const T*>(p.x) + lane_elems);
@@ -557,24 +477,13 @@ __global__ void __launch_bounds__(kStreamThreads, tiled_min_blocks(VEC, K)) k_ro
       else sp = xlane + (unsigned long long)(unsigned)s_u * ldxb;
 #pragma unroll
       for (int k = 0; k < K; ++k)
-        if (fm.ok[k]) cp_async_chunk<CB, L1>(dst + k * (32 * CB), sp + k * (32 * CB), keep);
+        if (fm.ok[k]) cp_async16<L1>(dst + k * (32 * CB), sp + k * (32 * CB), keep);
     }
     cp_async_commit();
   };
-#endif
 
   int pend = source_of(lane);                 // sources of segment 0
-  unsigned phase0 = 0, phase1 = 0;
-  (void)phase0; (void)phase1;
   if (Te > 0) {
-#if PNA_STREAM_TMA
-    issue_half(0, pend);
-    pend = source_of(H + lane);
-    if (H < Te) {
-      issue_half(1, pend);
-      pend = source_of(2 * H + lane);
-    }
-#else
     // fill the whole ring; segments past the end of the stream are copied too (row 0, never read): "one group per
     // segment" keeps wait_group<NST-1> exact
 #pragma unroll
@@ -582,7 +491,6 @@ __global__ void __launch_bounds__(kStreamThreads, tiled_min_blocks(VEC, K)) k_ro
       issue_half(s0, pend);
       pend = source_of((s0 + 1) * H + lane);
     }
-#endif
   }
   int stage = 0;        // ring segment that holds stream positions [n*H, n*H + H) being consumed
   int n_issued = NST;   // segments issued so far
@@ -625,12 +533,7 @@ __global__ void __launch_bounds__(kStreamThreads, tiled_min_blocks(VEC, K)) k_ro
         // segment = slots of this row inside the current half
         const int inhalf = q & (H - 1);
         if (inhalf == 0) {       // entering a segment: wait for its copies
-#if PNA_STREAM_TMA
-          if (stage) { mbar_wait(bar0 + 8, phase1); phase1 ^= 1; }
-          else { mbar_wait(bar0, phase0); phase0 ^= 1; }
-#else
           cp_async_wait<NST - 1>();    // all groups but the NST-1 newest (the segments still in flight) have landed
-#endif
         }
         const int seg = min(left, H - inhalf);
         unsigned sp = ring + (unsigned)(stage * H + inhalf) * SLOT + lane_off;
@@ -659,16 +562,8 @@ __global__ void __launch_bounds__(kStreamThreads, tiled_min_blocks(VEC, K)) k_ro
         q += seg;
         left -= seg;
         if ((q & (H - 1)) == 0 || q == Te) {   // segment fully consumed: refill it with the segment NST further on
-#if PNA_STREAM_TMA
-          __syncwarp();
-          if (n_issued * H < Te) {
-            issue_half(stage, pend);
-            pend = source_of((n_issued + 1) * H + lane);
-          }
-#else
           issue_half(stage, pend);             // (a group of unread copies past the end of the stream)
           pend = source_of((n_issued + 1) * H + lane);
-#endif
           ++n_issued;
           stage = (stage + 1 == NST) ? 0 : stage + 1;
         }
@@ -695,10 +590,7 @@ __global__ void __launch_bounds__(kStreamThreads, tiled_min_blocks(VEC, K)) k_ro
     }
     dg = dgN; rid = ridN;
   }
-#if !PNA_STREAM_TMA
-  if (n_fpass > 1 || p.work_ctr) { cp_async_wait<0>(); __syncwarp(); }    // the ring is refilled from its first segment
-#endif
- }  // feature passes
+  if (p.work_ctr) { cp_async_wait<0>(); __syncwarp(); }    // the next range refills the ring from its first segment
   }  // pa < pb
   if (!p.work_ctr) break;
   int g = 0;
@@ -897,31 +789,6 @@ __global__ void __launch_bounds__(kFinGroups * 32) k_hub_finalize(const KParams 
 }
 
 // ---- host dispatch -----------------------------------------------------------------------------------------
-// Feature-split streamed kernel for fp32 rows of 128 features (pna_aggregate_f32_fsplit.cu): 64-bit lane chunks,
-// two passes of 64 features.  Returns PNA_OK after launching, or > 0 when the shape is not one it takes.
-int launch_stream_fsplit_f32(const KParams& p, cudaStream_t st);
-// tuning knob (experiments only): PNA_B200_FEAT_SPLIT = "tiled2" | "stream2"
-static inline int feat_split_mode() {
-  static int mode = -1;
-  if (mode < 0) {
-    const char* e = getenv("PNA_B200_FEAT_SPLIT");
-    mode = !e ? 0 : (!strcmp(e, "tiled2") ? 1 : (!strcmp(e, "stream2") ? 2 : 0));
-  }
-  return mode;
-}
-
-// tuning knob (experiments only): PNA_B200_OVERSUB = CTAs launched per resident CTA slot of the streamed kernel (default 1:
-// a persistent grid).  > 1: more, shorter static ranges; the hardware hands the extra CTAs to the SMs that finish first.
-static inline int stream_oversubscription() {
-  static int v = 0;
-  if (v == 0) {
-    const char* e = getenv("PNA_B200_OVERSUB");
-    v = e ? atoi(e) : 1;
-    if (v < 1) v = 1;
-  }
-  return v;
-}
-
 template <typename T, int VEC, int G, int K, int U>
 static int launch_config(const KParams& p_in, cudaStream_t st) {
   constexpr int RPW = 32 / G;
@@ -942,19 +809,7 @@ static int launch_config(const KParams& p_in, cudaStream_t st) {
       // identity scaler only: the compact [N, A*F] result consumed by pna_linear_scaled_fwd
       const bool s1 = p.nS == 1 && (p.scodes & 0xfu) == PNA_SCALE_IDENTITY && p.nA == 4;
       const int cfg = (p.acodes & 0xffffu) != CfgMeanMaxMinStd::ACODES ? 0 : s3 ? 1 : s1 ? 2 : 0;
-      bool fsplit_done = false;
-      if constexpr (G == 32 && VEC == 4 && K == 1 && sizeof(T) == 4) {
-        if (feat_split_mode() == 2 && p.lrowptr != nullptr && p.col != nullptr && p.peer_x == nullptr && p.bias == nullptr &&
-            cfg == 1 && p.F == 128) {
-          p.hub_done = nullptr;
-          const int rc = launch_stream_fsplit_f32(p, st);
-          if (rc < 0) return rc;
-          fsplit_done = rc == 0;
-          if (fsplit_done) chunks_in_stream = p.n_view_rows > p.n_rows;
-        }
-      }
-      if (fsplit_done) {
-      } else if (G == 32 && VEC > 1 && p.lrowptr != nullptr && p.col != nullptr) {
+      if (G == 32 && VEC > 1 && p.lrowptr != nullptr && p.col != nullptr) {
        if constexpr (G == 32 && VEC > 1) {
         // streamed gather over the light view, persistent warps
         const bool b = p.bias != nullptr;
@@ -965,8 +820,8 @@ static int launch_config(const KParams& p_in, cudaStream_t st) {
     constexpr size_t smem = StreamGeom<T, VEC, K, DEPTH>::kSmem;                                                   \
     auto kern = k_rows_stream<T, VEC, K, CFG, B, DEPTH, FOLD, L1>;                                                     \
     static int resident = 0;  /* CTAs of this kernel that fit the device (every device of a process alike) */                \
-    if (resident == 0) {                                                                                           \
-      if (smem > 48 * 1024) PNA_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+    if (resident == 0) {  /* (static + dynamic shared memory of the K = 3 ring exceeds the 48 KB default) */       \
+      PNA_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));            \
       int dev = 0, sms = 0, nb = 0;                                                                                \
       PNA_CUDA_TRY(cudaGetDevice(&dev));                                                                           \
       PNA_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));                             \
@@ -974,7 +829,7 @@ static int launch_config(const KParams& p_in, cudaStream_t st) {
       resident = (nb > 0 ? nb : 1) * sms;                                                                          \
     }                                                                                                              \
     long long gxs = (slots + 8 * (kStreamThreads / 32) - 1) / (8 * (kStreamThreads / 32)); /* >= 8 rows per warp */ \
-    if (gxs > (long long)resident * stream_oversubscription()) gxs = (long long)resident * stream_oversubscription(); \
+    if (gxs > resident) gxs = resident;                                                                            \
     if (gxs < 1) gxs = 1;                                                                                          \
     if (p.work_ctr) {   /* dynamic tail: the last ~30 % of the partitions, if every warp still gets static work */  \
       const long long nw = gxs * (kStreamThreads / 32);                                                            \
@@ -1066,7 +921,6 @@ int launch_typed(const KParams& p, cudaStream_t st) {
   if (chunks <= 4) return launch_config<T, VEC, 4, 1, 4>(p, st);
   if (chunks <= 8) return launch_config<T, VEC, 8, 1, 4>(p, st);
   if (chunks <= 16) return launch_config<T, VEC, 16, 1, 4>(p, st);
-  if (chunks == 32 && feat_split_mode() == 1) return launch_config<T, VEC, 16, 1, 4>(p, st);   // two feature blocks (gridDim.y)
   if (chunks <= 32) return launch_config<T, VEC, 32, 1, 4>(p, st);
   if (chunks <= 64) return launch_config<T, VEC, 32, 2, 2>(p, st);
   if (chunks <= 96) return launch_config<T, VEC, 32, 3, 2>(p, st);
