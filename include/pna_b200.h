@@ -53,6 +53,16 @@ enum pna_aggr { PNA_AGGR_SUM = 0, PNA_AGGR_MEAN = 1, PNA_AGGR_MIN = 2, PNA_AGGR_
                    descriptors with peer_gathered or row_ids return PNA_ERR_UNSUPPORTED for them.  Rows at/above the split
                    threshold are merged in fixed chunk order (no atomics).  Rounding order: pna_b200/csrc/pna_aggregate_moments.cuh */
                 PNA_AGGR_MOMENT3 = 6, PNA_AGGR_MOMENT4 = 7, PNA_AGGR_MOMENT5 = 8,
+                /* weighted sums y = sum over slots of w_s m_s (models/pytorch/pna/aggregators.py:87-119), d == 0: 0:
+                     softmax:          w_s = exp(m_s - M) / Z,  M = max m,  Z = sum exp(m_t - M)
+                     softmin:          w_s = exp(M' - m_s) / Z', M' = min m (the reference's -softmax(-m))
+                     normalised_mean:  w_s = D_i^(-1/2) D_j^(-1/2), j = col[s], D_k = rowptr[k+1] - rowptr[k] of the SAME
+                                       CSR (0 weight where D_j == 0 or j >= n_rows); needs col != NULL.
+                   Taken by pna_aggregate_fwd, pna_aggregate_bwd and pna_aggregate_bwd_slots; pna_aggregate_bwd_coef and
+                   descriptors with peer_gathered or row_ids return PNA_ERR_UNSUPPORTED for them, as for the moments.
+                   Split rows are merged in fixed chunk order (no atomics).  Rounding order:
+                   pna_b200/csrc/pna_aggregate_weighted.cuh */
+                PNA_AGGR_SOFTMAX = 9, PNA_AGGR_SOFTMIN = 10, PNA_AGGR_NORMALISED_MEAN = 11,
                 PNA_AGGR_SKIP = 15 /* keep the column slot but do not write it: lets two calls with different edge
                                        sets / messages fill one output row (dense reference layer, where max/min and
                                        mean/std see different messages: models/pytorch/pna/aggregators.py:30-51) */ };

@@ -18,7 +18,7 @@ CUDA_SOURCES = [os.path.join(_HERE, "csrc", n) for n in
                 ("pna_aggregate.cu", "pna_aggregate_f32_vec.cu", "pna_aggregate_f32_scalar.cu", "pna_aggregate_bf16_vec.cu",
                  "pna_aggregate_bf16_scalar.cu", "pna_aggregate_bwd.cu", "pna_linear.cu", "pna_csr.cu", "pna_peer.cu", "pna_misc.cu")]
 CUDA_HEADERS = [os.path.join(_HERE, "csrc", n) for n in ("common.cuh", "pna_aggregate.cuh", "pna_aggregate_impl.cuh",
-                                                                   "pna_aggregate_moments.cuh")] + [
+                                                                   "pna_aggregate_moments.cuh", "pna_aggregate_weighted.cuh")] + [
     os.path.join(REPO_ROOT, "include", "pna_b200.h")]
 BUILD_DIR = os.path.join(_HERE, "csrc", "build")
 
@@ -35,7 +35,9 @@ AGGR_CODES = {"sum": 0, "mean": 1, "min": 2, "max": 3, "var": 4, "std": 5, "_ski
 # the central moments of the dense registry (PNA_AGGR_MOMENT3..5): a separate table, merged where the aggregation packs its
 # list, so that AGGR_CODES stays the set every flavour's layers accept
 MOMENTS = ("moment3", "moment4", "moment5")
-ALL_AGGR_CODES = {**AGGR_CODES, "moment3": 6, "moment4": 7, "moment5": 8}
+# the weighted sums of the dense registry (PNA_AGGR_SOFTMAX, _SOFTMIN, _NORMALISED_MEAN), in the same table
+WEIGHTED = ("softmax", "softmin", "normalised_mean")
+ALL_AGGR_CODES = {**AGGR_CODES, "moment3": 6, "moment4": 7, "moment5": 8, "softmax": 9, "softmin": 10, "normalised_mean": 11}
 SCALER_CODES = {"identity": 0, "amplification": 1, "attenuation": 2, "linear": 3, "inverse_linear": 4}
 FLAG_ZERO_ISOLATED, FLAG_SKIP_LIGHT, FLAG_SKIP_HUBS, FLAG_RELU_VAR, FLAG_GATHER_L1 = 1, 2, 4, 8, 16
 (QUERY_ABI_VERSION, QUERY_SM_ARCH, QUERY_DEFAULT_SPLIT, QUERY_DEFAULT_CHUNK, QUERY_DEVICE_SM_COUNT,

@@ -82,6 +82,11 @@ def aggregate_forward(gathered: torch.Tensor, csr: CSRGraph, aggregators: Names,
                (the ``torch.cat([x, out])`` of pna.py:131); ``self_divided`` tells whether tower t reads columns
                ``t*Ft:(t+1)*Ft`` (divide_input=True) or the same ``0:Ft`` (repeat, pna.py:126).
     """
+    if "normalised_mean" in _names(aggregators):
+        # its weight D_i^(-1/2) D_j^(-1/2) reads the source's degree from the same CSR: every gathered row must be a row of it
+        if messages_in_csr_order or peer is not None or gathered.size(0) != csr.n_nodes:
+            raise ValueError("normalised_mean needs gathered rows that are the CSR's own rows ([n_nodes, F], gathered through "
+                             "col): not messages in CSR order, a peer table, or a [local ; halo] row buffer")
     if not gathered.is_cuda:
         raise ValueError("pna_b200 kernels run on CUDA tensors only; there is no CPU fallback")
     if gathered.dtype not in _DTYPES:
@@ -227,9 +232,10 @@ def aggregate_backward(grad_out: torch.Tensor, gathered: torch.Tensor, csr: CSRG
     if deterministic:
         _backward_deterministic(d, grad_out, ld_go, gathered, csr, gg, gb, messages_in_csr_order)
         return gg, gb
-    # moments have no coefficient form (their per-slot gradient is a polynomial of degree k-1 in m): atomic path
+    # moments and the weighted sums have no coefficient form (their per-slot gradient is not c0 + c1 * m): atomic path
     if messages_in_csr_order or csr.n_edges == 0 or csr.sources_unique or backward_mode() == "atomic" \
-            or any(a in _lib.MOMENTS for a in _names(aggregators)) or 2 * _round_up(F, 4) > _lib.query(_lib.QUERY_MAX_FEATURES):
+            or any(a in _lib.MOMENTS + _lib.WEIGHTED for a in _names(aggregators)) \
+            or 2 * _round_up(F, 4) > _lib.query(_lib.QUERY_MAX_FEATURES):
         with torch.cuda.device(dev):
             _lib.check(_lib.lib().pna_aggregate_bwd(C.byref(d), grad_out.data_ptr(), ld_go, gg.data_ptr(), F, _ptr(gb), F,
                                                     torch.cuda.current_stream(dev).cuda_stream))
@@ -300,7 +306,8 @@ def backward_mode() -> str:
     transposed graph through the forward kernels, ``pna_aggregate_bwd_combine`` -- atomics only for min / max.  The
     coefficient path avoids the atomics that contend on hot source rows (power-law graphs), but regrouping sum_i (c0_i + c1_i x_j) into sum_i c0_i + x_j sum_i c1_i cancels badly where many rows have var ~ 0
     (2.6x the fp32 error of the per-edge evaluation on a power-law multigraph), so it stays opt-in.  Calls whose list contains a
-    moment aggregator take the atomic path under ``PNA_B200_BWD=coef``: a moment's gradient is not c0 + c1 * m.
+    moment aggregator, softmax, softmin or normalised_mean take the atomic path under ``PNA_B200_BWD=coef``: their gradient is
+    not c0 + c1 * m.
     Under ``torch.use_deterministic_algorithms(True)`` (``warn_only`` too) "deterministic", whatever PNA_B200_BWD says: per-slot
     gradients (``pna_aggregate_bwd_slots``) summed over the reversed edges by the forward kernel, no floating-point atomics,
     the same bits on every run."""

@@ -33,6 +33,51 @@ static int launch_moments_fwd(const MParams& p, cudaStream_t st) {
   return PNA_OK;
 }
 
+// The columns of one weighted aggregator (pna_aggregate_weighted.cuh), after the existing kernels and the moments.
+template <typename T>
+static int launch_weighted_fwd(const MParams& p, unsigned code, cudaStream_t st) {
+  const unsigned gy = (unsigned)((p.F + 31) / 32);
+  constexpr long long per_block = kMomThreads / 32;
+  if (!(p.flags & PNA_FLAG_SKIP_LIGHT)) {
+    const long long gx = (p.n_rows + per_block - 1) / per_block;
+    PNA_REQUIRE(gx <= 0x7fffffffll, PNA_ERR_UNSUPPORTED, "pna_aggregate_fwd: too many rows");
+    k_wsum_rows<T><<<dim3((unsigned)gx, gy), kMomThreads, 0, st>>>(p, code);
+    PNA_CUDA_TRY(cudaGetLastError());
+  }
+  if (!(p.flags & PNA_FLAG_SKIP_HUBS) && p.n_hubs > 0) {
+    const unsigned gc = (unsigned)((p.n_chunks + per_block - 1) / per_block), gh = (unsigned)((p.n_hubs + per_block - 1) / per_block);
+    if (code != PNA_AGGR_NORMALISED_MEAN) {
+      k_wsum_chunk_max<T, 4><<<dim3(gc, gy), kMomThreads, 0, st>>>(p, code);
+      PNA_CUDA_TRY(cudaGetLastError());
+      k_wsum_hub_max<4><<<dim3(gh, gy), kMomThreads, 0, st>>>(p);
+      PNA_CUDA_TRY(cudaGetLastError());
+    }
+    k_wsum_chunk_zs<T, 4><<<dim3(gc, gy), kMomThreads, 0, st>>>(p, code);
+    PNA_CUDA_TRY(cudaGetLastError());
+    k_wsum_hub_final<T><<<dim3(gh, gy), kMomThreads, 0, st>>>(p, code);
+    PNA_CUDA_TRY(cudaGetLastError());
+  }
+  return PNA_OK;
+}
+
+// The add-on aggregators after the existing kernels: the moments, then each weighted aggregator in turn (stream order,
+// so that each reuses hub_partials).
+template <typename T>
+static int launch_addons_fwd(const pna_agg_t* d, cudaStream_t st) {
+  const MParams mp = moment_params(d);
+  if (mp.orders) {
+    const int rc = launch_moments_fwd<T>(mp, st);
+    if (rc != PNA_OK) return rc;
+  }
+  const unsigned w = weighted_codes(d->aggr_codes, d->n_aggr);
+  for (unsigned c = PNA_AGGR_SOFTMAX; c <= PNA_AGGR_NORMALISED_MEAN; ++c) {
+    if (!((w >> (c - PNA_AGGR_SOFTMAX)) & 1u)) continue;
+    const int rc = launch_weighted_fwd<T>(mp, c, st);
+    if (rc != PNA_OK) return rc;
+  }
+  return PNA_OK;
+}
+
 }  // namespace pna
 
 using namespace pna;
@@ -49,15 +94,21 @@ extern "C" int pna_aggregate_fwd(const pna_agg_t* d, pna_stream_t stream) {
   PNA_REQUIRE(d->n_aggr >= 1 && d->n_aggr <= PNA_MAX_AGGR && d->n_scalers >= 1 && d->n_scalers <= PNA_MAX_SCALERS,
               PNA_ERR_BAD_ARG, "pna_aggregate_fwd: n_aggr=%d n_scalers=%d out of range", d->n_aggr, d->n_scalers);
   for (int a = 0; a < d->n_aggr; ++a)
-    PNA_REQUIRE(((d->aggr_codes >> (4 * a)) & 15u) <= PNA_AGGR_MOMENT5 || ((d->aggr_codes >> (4 * a)) & 15u) == PNA_AGGR_SKIP,
+    PNA_REQUIRE(((d->aggr_codes >> (4 * a)) & 15u) <= PNA_AGGR_NORMALISED_MEAN || ((d->aggr_codes >> (4 * a)) & 15u) == PNA_AGGR_SKIP,
                 PNA_ERR_BAD_ARG, "pna_aggregate_fwd: bad aggregator code");
   const bool moments = moment_orders(d->aggr_codes, d->n_aggr) != 0;
+  const unsigned weighted = weighted_codes(d->aggr_codes, d->n_aggr);
+  const bool addons = moments || weighted;
   PNA_REQUIRE(!moments || (!d->peer_gathered && !d->row_ids), PNA_ERR_UNSUPPORTED,
               "pna_aggregate_fwd: moment aggregators are not available with peer_gathered or row_ids");
+  PNA_REQUIRE(!weighted || (!d->peer_gathered && !d->row_ids), PNA_ERR_UNSUPPORTED,
+              "pna_aggregate_fwd: softmax / softmin / normalised_mean are not available with peer_gathered or row_ids");
   for (int s = 0; s < d->n_scalers; ++s)
     PNA_REQUIRE(((d->scaler_codes >> (4 * s)) & 15u) <= PNA_SCALE_INVERSE_LINEAR, PNA_ERR_BAD_ARG,
                 "pna_aggregate_fwd: bad scaler code");
   PNA_REQUIRE(d->dtype == PNA_F32 || d->dtype == PNA_BF16, PNA_ERR_UNSUPPORTED, "pna_aggregate_fwd: dtype %d", d->dtype);
+  PNA_REQUIRE(!((weighted >> (PNA_AGGR_NORMALISED_MEAN - PNA_AGGR_SOFTMAX)) & 1u) || d->col, PNA_ERR_UNSUPPORTED,
+              "pna_aggregate_fwd: normalised_mean needs col (the source of every slot)");
   if (d->n_rows == 0) return PNA_OK;
   PNA_REQUIRE(d->gathered && d->rowptr && d->out, PNA_ERR_BAD_ARG, "pna_aggregate_fwd: null gathered/rowptr/out");
   PNA_REQUIRE(d->split_threshold >= 2 && d->chunk_edges >= 1, PNA_ERR_BAD_ARG, "pna_aggregate_fwd: bad split/chunk");
@@ -75,7 +126,7 @@ extern "C" int pna_aggregate_fwd(const pna_agg_t* d, pna_stream_t stream) {
   p.F = d->n_feat; p.T = d->n_towers; p.Ft = d->n_feat / d->n_towers;
   p.has_self = d->self_feat ? 1 : 0;
   p.nA = d->n_aggr; p.nS = d->n_scalers; p.scodes = d->scaler_codes;
-  p.acodes = moments ? strip_moments(d->aggr_codes, d->n_aggr) : d->aggr_codes;   // the moment kernels write those columns
+  p.acodes = addons ? strip_addons(d->aggr_codes, d->n_aggr) : d->aggr_codes;   // the add-on kernels write those columns
   p.Wt = (p.has_self + p.nA * p.nS) * p.Ft;
   p.avg_log = d->avg_log; p.avg_lin = d->avg_lin;
   p.flags = d->flags; p.split = d->split_threshold; p.chunk = d->chunk_edges;
@@ -117,7 +168,6 @@ extern "C" int pna_aggregate_fwd(const pna_agg_t* d, pna_stream_t stream) {
   } else {
     rc = vec_ok ? launch_typed<__nv_bfloat16, 8>(p, st) : launch_typed<__nv_bfloat16, 1>(p, st);
   }
-  if (rc != PNA_OK || !moments) return rc;
-  const MParams mp = moment_params(d);
-  return d->dtype == PNA_F32 ? launch_moments_fwd<float>(mp, st) : launch_moments_fwd<__nv_bfloat16>(mp, st);
+  if (rc != PNA_OK || !addons) return rc;
+  return d->dtype == PNA_F32 ? launch_addons_fwd<float>(d, st) : launch_addons_fwd<__nv_bfloat16>(d, st);
 }

@@ -388,3 +388,4 @@ __device__ __forceinline__ void finalize_row_ds(const KParams& p, const FeatMap<
 }  // namespace pna
 
 #include "pna_aggregate_moments.cuh"
+#include "pna_aggregate_weighted.cuh"

@@ -584,6 +584,54 @@ static int launch_moments_bwd(const MParams& p, cudaStream_t st) {
   return PNA_OK;
 }
 
+// The term of one weighted aggregator in every slot's gradient (pna_aggregate_weighted.cuh), after the moments'.
+template <typename T, bool SLOTS>
+static int launch_weighted_bwd(const MParams& p, unsigned code, cudaStream_t st) {
+  const unsigned gy = (unsigned)((p.f1 - p.f0 + 31) / 32);
+  constexpr long long per_block = kMomThreads / 32;
+  const long long gx = (p.n_rows + per_block - 1) / per_block;
+  PNA_REQUIRE(gx <= 0x7fffffffll, PNA_ERR_UNSUPPORTED, "pna_aggregate_bwd: too many rows");
+  k_wsum_bwd_rows<T, SLOTS><<<dim3((unsigned)gx, gy), kMomThreads, 0, st>>>(p, code);
+  PNA_CUDA_TRY(cudaGetLastError());
+  if (p.n_hubs > 0) {
+    const unsigned gc = (unsigned)((p.n_chunks + per_block - 1) / per_block), gh = (unsigned)((p.n_hubs + per_block - 1) / per_block);
+    if (code != PNA_AGGR_NORMALISED_MEAN) {
+      k_wsum_chunk_max<T, 6><<<dim3(gc, gy), kMomThreads, 0, st>>>(p, code);
+      PNA_CUDA_TRY(cudaGetLastError());
+      k_wsum_hub_max<6><<<dim3(gh, gy), kMomThreads, 0, st>>>(p);
+      PNA_CUDA_TRY(cudaGetLastError());
+      k_wsum_chunk_zs<T, 6><<<dim3(gc, gy), kMomThreads, 0, st>>>(p, code);
+      PNA_CUDA_TRY(cudaGetLastError());
+    }
+    k_wsum_bwd_hub_coef<T><<<dim3(gh, gy), kMomThreads, 0, st>>>(p, code);
+    PNA_CUDA_TRY(cudaGetLastError());
+    k_wsum_bwd_chunk_grad<T, SLOTS><<<dim3(gc, gy), kMomThreads, 0, st>>>(p, code);
+    PNA_CUDA_TRY(cudaGetLastError());
+    if (p.gb) {
+      k_mom_bwd_hub_bias<6><<<dim3(gh, gy), kMomThreads, 0, st>>>(p);
+      PNA_CUDA_TRY(cudaGetLastError());
+    }
+  }
+  return PNA_OK;
+}
+
+// The add-on aggregators' terms: the moments, then each weighted aggregator in turn (stream order: each reuses
+// hub_partials).
+template <typename T, bool SLOTS>
+static int launch_addons_bwd(const pna_agg_t* d, const MParams& mp, cudaStream_t st) {
+  if (mp.orders) {
+    const int rc = launch_moments_bwd<T, SLOTS>(mp, st);
+    if (rc != PNA_OK) return rc;
+  }
+  const unsigned w = weighted_codes(d->aggr_codes, d->n_aggr);
+  for (unsigned c = PNA_AGGR_SOFTMAX; c <= PNA_AGGR_NORMALISED_MEAN; ++c) {
+    if (!((w >> (c - PNA_AGGR_SOFTMAX)) & 1u)) continue;
+    const int rc = launch_weighted_bwd<T, SLOTS>(mp, c, st);
+    if (rc != PNA_OK) return rc;
+  }
+  return PNA_OK;
+}
+
 // ---- phase 3 of the coefficient path: grad_gathered[j] += S0[j] + gathered[j] * S1[j] ------------------------------------
 // sums[j] = [S0 | S1] (S1 at column c1): the 'sum' of the coefficient rows over the out-edges of source row j.
 template <typename T>
@@ -630,6 +678,16 @@ static int bwd_entry(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_o
               "pna_aggregate_bwd_coef: moment aggregators have no coefficient form; use pna_aggregate_bwd or pna_aggregate_bwd_slots");
   PNA_REQUIRE(!moments || (!d->peer_gathered && !d->row_ids), PNA_ERR_UNSUPPORTED,
               "pna_aggregate_bwd: moment aggregators are not available with peer_gathered or row_ids");
+  const unsigned weighted = weighted_codes(d->aggr_codes, d->n_aggr);
+  const bool addons = moments || weighted;
+  // softmax / softmin: p_j (1 + m_j - y) is not linear in m_j; normalised_mean's weight depends on the source's degree
+  PNA_REQUIRE(!weighted || !coef, PNA_ERR_UNSUPPORTED,
+              "pna_aggregate_bwd_coef: softmax / softmin / normalised_mean have no coefficient form; use pna_aggregate_bwd or "
+              "pna_aggregate_bwd_slots");
+  PNA_REQUIRE(!weighted || (!d->peer_gathered && !d->row_ids), PNA_ERR_UNSUPPORTED,
+              "pna_aggregate_bwd: softmax / softmin / normalised_mean are not available with peer_gathered or row_ids");
+  PNA_REQUIRE(!((weighted >> (PNA_AGGR_NORMALISED_MEAN - PNA_AGGR_SOFTMAX)) & 1u) || d->col, PNA_ERR_UNSUPPORTED,
+              "pna_aggregate_bwd: normalised_mean needs col (the source of every slot)");
   if (d->n_rows == 0) return PNA_OK;
   PNA_REQUIRE(d->gathered && d->rowptr && grad_out && (slots || grad_gathered), PNA_ERR_BAD_ARG, "pna_aggregate_bwd: null pointer");
   PNA_REQUIRE(d->peer_gathered == nullptr, PNA_ERR_UNSUPPORTED, "pna_aggregate_bwd: peer-memory graphs are forward-only");
@@ -649,7 +707,7 @@ static int bwd_entry(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_o
   p.F = d->n_feat; p.T = d->n_towers; p.Ft = d->n_feat / d->n_towers;
   p.has_self = d->self_feat ? 1 : 0;
   p.nA = d->n_aggr; p.nS = d->n_scalers; p.scodes = d->scaler_codes;
-  p.acodes = moments ? strip_moments(d->aggr_codes, d->n_aggr) : d->aggr_codes;   // the moment kernels add their term
+  p.acodes = addons ? strip_addons(d->aggr_codes, d->n_aggr) : d->aggr_codes;   // the add-on kernels add their term
   p.Wt = (p.has_self + p.nA * p.nS) * p.Ft;
   p.avg_log = d->avg_log; p.avg_lin = d->avg_lin;
   p.flags = d->flags; p.split = d->split_threshold; p.chunk = d->chunk_edges;
@@ -688,17 +746,17 @@ static int bwd_entry(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_o
     if (f32) rc = vec_ok ? launch_bwd_typed<float, 4, false>(b, st) : launch_bwd_typed<float, 1, false>(b, st);
     else rc = vec_ok ? launch_bwd_typed<__nv_bfloat16, 8, false>(b, st) : launch_bwd_typed<__nv_bfloat16, 1, false>(b, st);
   }
-  if (rc != PNA_OK || !moments) return rc;
+  if (rc != PNA_OK || !addons) return rc;
   MParams mp = moment_params(d);
   mp.go = grad_out; mp.ldgo = ld_grad_out;
   mp.gb = grad_row_bias; mp.ldgb = ld_grad_row_bias;
   if (slots) {
     mp.gs = grad_slots; mp.ldgs = ld_grad_slots;
     mp.f0 = f_begin; mp.f1 = f_begin + f_count;
-    return f32 ? launch_moments_bwd<float, true>(mp, st) : launch_moments_bwd<__nv_bfloat16, true>(mp, st);
+    return f32 ? launch_addons_bwd<float, true>(d, mp, st) : launch_addons_bwd<__nv_bfloat16, true>(d, mp, st);
   }
   mp.gg = grad_gathered; mp.ldgg = ld_grad_gathered;
-  return f32 ? launch_moments_bwd<float, false>(mp, st) : launch_moments_bwd<__nv_bfloat16, false>(mp, st);
+  return f32 ? launch_addons_bwd<float, false>(d, mp, st) : launch_addons_bwd<__nv_bfloat16, false>(d, mp, st);
 }
 
 extern "C" int pna_aggregate_bwd(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_out, float* grad_gathered,

@@ -46,13 +46,6 @@ inline unsigned moment_orders(unsigned codes, int n_aggr) {
   return m;
 }
 
-// the list with every moment code replaced by PNA_AGGR_SKIP: what the existing kernels run
-inline unsigned strip_moments(unsigned codes, int n_aggr) {
-  for (int a = 0; a < n_aggr; ++a)
-    if (moment_order((codes >> (4 * a)) & 15u)) codes |= 15u << (4 * a);
-  return codes;
-}
-
 struct MParams {
   const void* x; long long ldx;
   const int* rowptr; const int* col;

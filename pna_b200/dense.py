@@ -13,13 +13,22 @@ aggregators.py:39,51) while ``mean/std/sum`` reduce over dim 2, so for node v
 Two kernel calls fill one output row (PNA_AGGR_SKIP keeps the other call's column slots).
 ``self_loop=True`` aggregates over adj + I while the scalers keep the loop-free row degree (``pna_agg_t.scaler_degree``);
 ``var`` is clamped at 0 as the reference does (PNA_FLAG_RELU_VAR).
-Restrictions (documented, not silent): 0/1 adjacency (the reference's weighted sums are not reproduced), aggregators
-mean/max/min/std/sum/var/moment3/moment4/moment5, and -- unlike the reference, which divides by zero -- isolated nodes get
-PyG semantics (a moment of a row without neighbours is 0).
+Restrictions (documented, not silent): 0/1 adjacency (the reference's weighted sums are not reproduced), and -- unlike
+the reference, which divides by zero -- isolated nodes get PyG semantics (a moment of a row without neighbours is 0).
+Every name of the reference registry (models/pytorch/pna/aggregators.py:149-152) is taken.
 The moments reduce over dim 2 like mean/std (self first).  ``self_loop=True`` with a moment raises NotImplementedError:
 the reference's ``aggregate_moment`` adds I to adj and then calls ``aggregate_mean(..., self_loop=True)``, which adds I
 again, so its moments are centred on a mean that counts the self loop twice -- not a central moment of any edge set the
 kernel can be given.
+softmax / softmin / normalised_mean also reduce over dim 2 (self first) and take ``self_loop=True`` (the reference adds I
+once).  Where they deliberately differ from the reference:
+  * a row without neighbours gives 0 (the reference: 0/0 = NaN for softmax and softmin);
+  * softmax / softmin are evaluated shifted by the row's max / min, so they stay finite where the reference's unshifted
+    exp overflows (messages above ~88.7) or underflows to 0/0;
+  * normalised_mean weighs with D_k^(-1/2) of the aggregated row degrees (adj + I with ``self_loop``); a graph with an
+    isolated node makes the reference's every row NaN (inf * 0 in its diagonal matmul), here that node just has weight 0.
+``identity`` is X_ii = pretrans([h_i, h_i]) whatever adj says: no kernel call, its column slots are filled here (both
+paths, autograd for its gradient) with the kernels' scaler factors of the loop-free row degree.
 """
 from __future__ import annotations
 
@@ -30,7 +39,7 @@ from .aggregate import aggregate_forward, pna_aggregate
 from .csr import build_csr, tensor_version
 from .nn_blocks import FCLayer, MLP
 
-_SELF_FIRST = ("mean", "std", "sum", "var", "moment3", "moment4", "moment5")
+_SELF_FIRST = ("mean", "std", "sum", "var", "moment3", "moment4", "moment5", "softmax", "softmin", "normalised_mean")
 _MOMENTS = ("moment3", "moment4", "moment5")
 _NBR_FIRST = ("max", "min")
 
@@ -89,7 +98,7 @@ class PNALayer(nn.Module):
         assert out_features % towers == 0
         self.aggregators, self.scalers = list(aggregators), list(scalers)
         for a in self.aggregators:
-            if a not in _SELF_FIRST + _NBR_FIRST:
+            if a not in _SELF_FIRST + _NBR_FIRST + ("identity",):
                 raise KeyError(f"aggregator {a!r} is not available on the CUDA path")
         if self_loop and any(a in _MOMENTS for a in self.aggregators):
             raise NotImplementedError("dense PNALayer: moment aggregators with self_loop=True are not supported (the reference "
@@ -117,8 +126,9 @@ class PNALayer(nn.Module):
             Wa, Wb = torch.cat(Wa, 0), torch.cat(Wb, 0)
         return h @ Wa.t(), h @ Wb.t(), b
 
-    def _second_call_columns(self, width, a2, device):
-        """bool [width]: output columns produced by the max/min call (per tower: self block, then S x A blocks of F_t)."""
+    def _columns(self, width, a2, device):
+        """bool [width]: output columns of the list positions of ``a2`` that are not "_skip" (per tower: self block, then
+        S x A blocks of F_t) -- those of the max/min call, or of ``identity``."""
         T, Ft = len(self.towers), self.input_tower
         A, S = len(self.aggregators), len(self.scalers)
         m = torch.zeros(T, 1 + S * A, Ft, dtype=torch.bool)
@@ -153,12 +163,32 @@ class PNALayer(nn.Module):
             out = pna_aggregate(Bm + b, graphs.row, a1, self.scalers, self.avg_d, row_bias=A, **common)
             if any(a != "_skip" for a in a2):
                 out2 = pna_aggregate(A + b, graphs.colwise, a2, self.scalers, self.avg_d, row_bias=Bm, **common)
-                out = torch.where(self._second_call_columns(out.size(1), a2, h.device), out2, out) if both else out2
+                out = torch.where(self._columns(out.size(1), a2, h.device), out2, out) if both else out2
+        if "identity" in self.aggregators:
+            # X_ii = pretrans([h_i, h_i]) per tower, in every scaler's slot; autograd carries its gradient
+            ident = [a if a == "identity" else "_skip" for a in self.aggregators]
+            out = torch.where(self._columns(out.size(1), ident, h.device), self._identity_block(A + Bm + b, graphs), out)
         # both calls scale with the ROW degree D = adj.sum(-1) of the loop-free adjacency (scaler_degree), as
         # models/pytorch/pna/scalers.py:13,21 does, whatever edge set the aggregators reduced over
         out = out.view(B * N, T, -1)
         y = torch.cat([tw.posttrans(out[:, t]) for t, tw in enumerate(self.towers)], dim=1)
         return self.mixing_network(y).view(B, N, -1)
+
+    def _identity_block(self, x_id, graphs):
+        """[B*N, T * (1 + S*A) * F_t]: x_id's tower slice times each scaler's factor in every (scaler, aggregator) slot; the
+        factors are the aggregation epilogue's (common.cuh deg_scales: attenuation / inverse_linear are 1 where D == 0)."""
+        T, Ft = len(self.towers), self.input_tower
+        A, S = len(self.aggregators), len(self.scalers)
+        D = graphs.scaler_degree.to(x_id.dtype)
+        lg = torch.log(D + 1)
+        one = torch.ones_like(D)
+        avg_log, avg_lin = self.avg_d["log"], self.avg_d.get("lin", 1.0)
+        fac = {"identity": one, "amplification": lg / avg_log, "attenuation": torch.where(D > 0, avg_log / lg, one),
+               "linear": D / avg_lin, "inverse_linear": torch.where(D > 0, avg_lin / D, one)}
+        f = torch.stack([fac[s_] for s_ in self.scalers], 1)                         # [B*N, S]
+        v = x_id.view(-1, T, 1, 1, Ft) * f.view(-1, 1, S, 1, 1)                      # [B*N, T, S, 1, F_t]
+        v = v.expand(-1, T, S, A, Ft).reshape(-1, T, S * A, Ft)
+        return torch.cat([torch.zeros_like(v[:, :, :1]), v], 2).reshape(x_id.size(0), -1)
 
     def __repr__(self):
         return f"{self.__class__.__name__} ({self.in_features} -> {self.out_features})"
