@@ -56,8 +56,9 @@ enum pna_aggr { PNA_AGGR_SUM = 0, PNA_AGGR_MEAN = 1, PNA_AGGR_MIN = 2, PNA_AGGR_
                 /* weighted sums y = sum over slots of w_s m_s (models/pytorch/pna/aggregators.py:87-119), d == 0: 0:
                      softmax:          w_s = exp(m_s - M) / Z,  M = max m,  Z = sum exp(m_t - M)
                      softmin:          w_s = exp(M' - m_s) / Z', M' = min m (the reference's -softmax(-m))
-                     normalised_mean:  w_s = D_i^(-1/2) D_j^(-1/2), j = col[s], D_k = rowptr[k+1] - rowptr[k] of the SAME
-                                       CSR (0 weight where D_j == 0 or j >= n_rows); needs col != NULL.
+                     normalised_mean:  w_s = D_i^(-1/2) D_j^(-1/2), j = col[s] (or degree_col[s] when given),
+                                       D_k = rowptr[k+1] - rowptr[k] of the SAME CSR (0 weight where D_j == 0 or
+                                       j >= n_rows); needs col != NULL or degree_col != NULL.
                    Taken by pna_aggregate_fwd, pna_aggregate_bwd and pna_aggregate_bwd_slots; pna_aggregate_bwd_coef and
                    descriptors with peer_gathered or row_ids return PNA_ERR_UNSUPPORTED for them, as for the moments.
                    Split rows are merged in fixed chunk order (no atomics).  Rounding order:
@@ -244,6 +245,11 @@ typedef struct pna_agg {
    * this counter, so warps that finish their static range early take over work from slow ones.  Not to be shared by
    * concurrent calls.  NULL: fully static assignment. */
   int32_t* work_counter;
+  /* optional int32 [n_edges]: for normalised_mean, the node whose row degree (rowptr[k+1] - rowptr[k] of this CSR) weighs
+   * each slot, in place of col[slot].  It lets normalised_mean run on messages already in CSR order (col == NULL): the
+   * dense layer with pretrans_layers >= 2 passes the row CSR's own col here.  Read by no other aggregator.  NULL: the
+   * slot's col entry (and normalised_mean needs col). */
+  const int32_t* degree_col;
 } pna_agg_t;
 
 int pna_aggregate_fwd(const pna_agg_t* desc, pna_stream_t stream);
@@ -293,6 +299,27 @@ int pna_aggregate_bwd_combine(const float* coef_sums, int64_t ld_sums, int32_t c
 int pna_aggregate_bwd_slots(const pna_agg_t* desc, const void* grad_out, int64_t ld_grad_out, int32_t f_begin, int32_t f_count,
                             float* grad_slots, int64_t ld_grad_slots, float* grad_row_bias, int64_t ld_grad_row_bias,
                             pna_stream_t stream);
+
+/* ---- the per-edge pretrans MLP of the dense layer with pretrans_layers = L >= 2 (models/layers.py:200-229) ------------
+ * For every slot s of a destination-sorted CSR (row i, source j = col[s]) and tower t (all fp32, row-major, contiguous,
+ * TF = n_towers * width):
+ *   z_1 = relu(a[i, t] + b[j, t] + bias1[t]),  z_k = relu(W_k[t] z_(k-1) + b_k[t]) (k = 2..L-1),
+ *   messages[s, t] = W_L[t] z_(L-1) + b_L[t]                                                   [n_edges, TF]
+ * a [n_rows, TF] is the destination half of the first layer's product, b [n_src, TF] the source half, bias1 [TF];
+ * weight [(L-1), n_towers, width, width] (nn.Linear's [out, in]) and bias [(L-1), n_towers, width] hold layers 2..L.
+ * activations (nullable) [(L-1), n_edges, TF] receives z_1 .. z_(L-1) for the backward.
+ * pna_edge_mlp_bwd: grad_pre [(L-1), n_edges, TF] receives G_1 .. G_(L-1), the gradients of the pre-activations of layers
+ * 1 .. L-1 (G_L is grad_messages):  G_(k-1) = (W_k[t]^T G_k) * [z_(k-1) > 0].  Weight / bias gradients and the
+ * gradients of a and b are the caller's (G_k^T z_(k-1), sums of G_k; sums of G_1 over rows and over sources).
+ * One thread per (slot, tower), no atomics: every value is a fixed function of its inputs.  n_layers < 2, width < 1,
+ * n_towers < 1 or a null pointer (with n_edges > 0): PNA_ERR_BAD_ARG; width > PNA_EDGE_MLP_MAX_WIDTH:
+ * PNA_ERR_UNSUPPORTED.  Rounding order: pna_b200/csrc/pna_edge_mlp.cu */
+#define PNA_EDGE_MLP_MAX_WIDTH 64
+int pna_edge_mlp_fwd(const int32_t* rowptr, const int32_t* col, int64_t n_rows, int64_t n_edges, const float* a, const float* b,
+                     const float* bias1, const float* weight, const float* bias, int32_t n_layers, int32_t n_towers,
+                     int32_t width, float* messages, float* activations, pna_stream_t stream);
+int pna_edge_mlp_bwd(const float* grad_messages, const float* activations, const float* weight, int64_t n_edges,
+                     int32_t n_layers, int32_t n_towers, int32_t width, float* grad_pre, pna_stream_t stream);
 
 /* ---- halo rows for the destination-partitioned multi-GPU path (north_star: "single NCCL all-to-all for halo
  * source features per layer"): dst[i, :] = src[idx[i], :], n_feat elements per row.  Used to pack the send buffer. */

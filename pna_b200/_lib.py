@@ -16,7 +16,8 @@ REPO_ROOT = os.path.dirname(_HERE)
 LIB_PATH = os.environ.get("PNA_B200_LIB") or os.path.join(_HERE, "libpna_sm90.so")   # env override: tuning builds only
 CUDA_SOURCES = [os.path.join(_HERE, "csrc", n) for n in
                 ("pna_aggregate.cu", "pna_aggregate_f32_vec.cu", "pna_aggregate_f32_scalar.cu", "pna_aggregate_bf16_vec.cu",
-                 "pna_aggregate_bf16_scalar.cu", "pna_aggregate_bwd.cu", "pna_linear.cu", "pna_csr.cu", "pna_peer.cu", "pna_misc.cu")]
+                 "pna_aggregate_bf16_scalar.cu", "pna_aggregate_bwd.cu", "pna_linear.cu", "pna_csr.cu", "pna_peer.cu", "pna_misc.cu",
+                 "pna_edge_mlp.cu")]
 CUDA_HEADERS = [os.path.join(_HERE, "csrc", n) for n in ("common.cuh", "pna_aggregate.cuh", "pna_aggregate_impl.cuh",
                                                                    "pna_aggregate_moments.cuh", "pna_aggregate_weighted.cuh")] + [
     os.path.join(REPO_ROOT, "include", "pna_b200.h")]
@@ -42,12 +43,14 @@ SCALER_CODES = {"identity": 0, "amplification": 1, "attenuation": 2, "linear": 3
 FLAG_ZERO_ISOLATED, FLAG_SKIP_LIGHT, FLAG_SKIP_HUBS, FLAG_RELU_VAR, FLAG_GATHER_L1 = 1, 2, 4, 8, 16
 (QUERY_ABI_VERSION, QUERY_SM_ARCH, QUERY_DEFAULT_SPLIT, QUERY_DEFAULT_CHUNK, QUERY_DEVICE_SM_COUNT,
  QUERY_MAX_FEATURES, QUERY_SIZEOF_CSR, QUERY_SIZEOF_AGG) = range(8)
+EDGE_MLP_MAX_WIDTH = 64      # PNA_EDGE_MLP_MAX_WIDTH
 
 # every symbol the header declares (checked by tests/test_abi.py)
 EXPORTED_SYMBOLS = ("pna_csr_workspace_bytes", "pna_csr_build", "pna_csr_light_view", "pna_csr_light_view_workspace_bytes", "pna_aggregate_fwd", "pna_aggregate_bwd",
                     "pna_aggregate_bwd_coef", "pna_aggregate_bwd_combine", "pna_aggregate_bwd_slots",
                     "pna_gather_rows", "pna_halo_pull", "pna_halo_grad_pull", "pna_peer_barrier", "pna_linear_fwd", "pna_linear_scaled_fwd", "pna_row_scales", "pna_linear_workspace_bytes",
-                    "pna_linear_bwd_workspace_bytes", "pna_linear_bwd_data", "pna_linear_bwd_weight", "pna_query", "pna_last_error")
+                    "pna_linear_bwd_workspace_bytes", "pna_linear_bwd_data", "pna_linear_bwd_weight", "pna_edge_mlp_fwd",
+                    "pna_edge_mlp_bwd", "pna_query", "pna_last_error")
 
 
 class PnaError(RuntimeError):
@@ -93,6 +96,7 @@ class AggStruct(C.Structure):
         ("light_rowptr", C.c_void_p), ("light_deg", C.c_void_p), ("light_col", C.c_void_p), ("part", C.c_void_p),
         ("n_part", C.c_int32), ("n_view_rows", C.c_int64), ("peer_gathered", C.c_void_p), ("peer_shift", C.c_int32),
         ("max_degree", C.c_int32), ("hub_done", C.c_void_p), ("scaler_degree", C.c_void_p), ("work_counter", C.c_void_p),
+        ("degree_col", C.c_void_p),
     ]
 
 
@@ -205,6 +209,12 @@ def lib() -> C.CDLL:
                                             C.c_int32, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]
         L.pna_row_scales.restype = C.c_int
         L.pna_row_scales.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_uint32, C.c_float, C.c_float, C.c_void_p, C.c_void_p]
+        L.pna_edge_mlp_fwd.restype = C.c_int
+        L.pna_edge_mlp_fwd.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.pna_edge_mlp_bwd.restype = C.c_int
+        L.pna_edge_mlp_bwd.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                       C.c_void_p]
         abi = L.pna_query(QUERY_ABI_VERSION)
         if abi != ABI_VERSION:
             raise ImportError(f"{LIB_PATH} has ABI version {abi}, this package needs {ABI_VERSION}: rebuild it")

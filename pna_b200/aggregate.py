@@ -57,6 +57,12 @@ def _check_scaler_degree(t: torch.Tensor, n_rows: int, dev) -> torch.Tensor:
     return t
 
 
+def _check_degree_col(t: torch.Tensor, n_edges: int, dev) -> torch.Tensor:
+    if t.dtype != torch.int32 or t.device != dev or t.numel() != n_edges or not t.is_contiguous():
+        raise ValueError("degree_col must be a contiguous int32 [n_edges] tensor on the same device")
+    return t
+
+
 def fold_finalize_enabled() -> bool:
     """PNA_B200_FOLD_FINALIZE=1: the warp that completes a split row also finalizes it (one launch per call)."""
     return os.environ.get("PNA_B200_FOLD_FINALIZE", "0") == "1"
@@ -72,7 +78,8 @@ def aggregate_forward(gathered: torch.Tensor, csr: CSRGraph, aggregators: Names,
                       messages_in_csr_order: bool = False, zero_isolated: bool = False, relu_var: bool = False,
                       out: Optional[torch.Tensor] = None, row_ids: Optional[torch.Tensor] = None,
                       skip_light: bool = False, skip_hubs: bool = False, view=None, peer=None,
-                      scaler_degree: Optional[torch.Tensor] = None, gather_l1: Optional[bool] = None) -> torch.Tensor:
+                      scaler_degree: Optional[torch.Tensor] = None, gather_l1: Optional[bool] = None,
+                      degree_col: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Run the CUDA aggregation (no autograd).  Returns ``[N, towers * (has_self + S*A) * Ft]``.
 
     gathered : [n_src, F] rows that are gathered through ``csr.col`` (x for PNAConvSimple; V = x W_j^T + b for
@@ -81,12 +88,16 @@ def aggregate_forward(gathered: torch.Tensor, csr: CSRGraph, aggregators: Names,
     self_feat: optional node features copied to the front of every tower block of the output row
                (the ``torch.cat([x, out])`` of pna.py:131); ``self_divided`` tells whether tower t reads columns
                ``t*Ft:(t+1)*Ft`` (divide_input=True) or the same ``0:Ft`` (repeat, pna.py:126).
+    degree_col: optional int32 [E]: for normalised_mean, the row of this CSR whose degree weighs each slot (in place of
+               ``col``) -- what lets it run on messages in CSR order (pna_agg_t.degree_col).
     """
     if "normalised_mean" in _names(aggregators):
-        # its weight D_i^(-1/2) D_j^(-1/2) reads the source's degree from the same CSR: every gathered row must be a row of it
-        if messages_in_csr_order or peer is not None or gathered.size(0) != csr.n_nodes:
+        # its weight D_i^(-1/2) D_j^(-1/2) reads the source's degree from the same CSR: every gathered row must be a row of
+        # it, or degree_col names that row per slot
+        if peer is not None or (degree_col is None and (messages_in_csr_order or gathered.size(0) != csr.n_nodes)):
             raise ValueError("normalised_mean needs gathered rows that are the CSR's own rows ([n_nodes, F], gathered through "
-                             "col): not messages in CSR order, a peer table, or a [local ; halo] row buffer")
+                             "col) or degree_col: not messages in CSR order without degree_col, a peer table, or a "
+                             "[local ; halo] row buffer")
     if not gathered.is_cuda:
         raise ValueError("pna_b200 kernels run on CUDA tensors only; there is no CPU fallback")
     if gathered.dtype not in _DTYPES:
@@ -146,6 +157,8 @@ def aggregate_forward(gathered: torch.Tensor, csr: CSRGraph, aggregators: Names,
         row_ids=_ptr(row_ids), n_row_ids=0 if row_ids is None else int(row_ids.numel()))
     if scaler_degree is not None:
         d.scaler_degree = _check_scaler_degree(scaler_degree, N, dev).data_ptr()
+    if degree_col is not None:
+        d.degree_col = _check_degree_col(degree_col, csr.n_edges, dev).data_ptr()
     if view is None and row_ids is None and _dynamic_tail(csr):
         d.work_counter = _ptr(csr.work_counter())      # the whole graph in one launch: dynamic tail of the streamed kernel
     if view is None and row_ids is None:
@@ -193,7 +206,8 @@ def row_scales(csr: CSRGraph, scalers: Names, avg_deg: Mapping[str, float]) -> t
 def aggregate_backward(grad_out: torch.Tensor, gathered: torch.Tensor, csr: CSRGraph, aggregators: Names, scalers: Names,
                        avg_deg: Mapping[str, float], *, towers: int = 1, row_bias: Optional[torch.Tensor] = None,
                        has_self: bool = False, messages_in_csr_order: bool = False, need_bias_grad: bool = False,
-                       relu_var: bool = False, scaler_degree: Optional[torch.Tensor] = None):
+                       relu_var: bool = False, scaler_degree: Optional[torch.Tensor] = None,
+                       degree_col: Optional[torch.Tensor] = None):
     """Gradient of the aggregation w.r.t. ``gathered`` (and ``row_bias``) through ``pna_aggregate_bwd`` (fp32 results)."""
     dev = gathered.device
     gathered = _rows2d(gathered, "gathered")
@@ -224,6 +238,8 @@ def aggregate_backward(grad_out: torch.Tensor, gathered: torch.Tensor, csr: CSRG
         n_hubs=csr.n_hubs, n_chunks=csr.n_chunks)
     if scaler_degree is not None:
         d.scaler_degree = _check_scaler_degree(scaler_degree, N, dev).data_ptr()
+    if degree_col is not None:
+        d.degree_col = _check_degree_col(degree_col, csr.n_edges, dev).data_ptr()
     scratch = None
     if csr.n_hubs:   # per-chunk statistics + per-split-row coefficients
         scratch = torch.empty(((csr.n_chunks + csr.n_hubs) * 6, F), dtype=torch.float32, device=dev)
@@ -319,24 +335,24 @@ def backward_mode() -> str:
 class _PNAAggregate(torch.autograd.Function):
     @staticmethod
     def forward(ctx, gathered, row_bias, self_feat, csr, aggregators, scalers, avg_deg, towers, self_divided,
-                messages_in_csr_order, zero_isolated, relu_var=False, scaler_degree=None):
+                messages_in_csr_order, zero_isolated, relu_var=False, scaler_degree=None, degree_col=None):
         out = aggregate_forward(gathered, csr, aggregators, scalers, avg_deg, towers=towers, row_bias=row_bias,
                                 self_feat=self_feat, self_divided=self_divided,
                                 messages_in_csr_order=messages_in_csr_order, zero_isolated=zero_isolated, relu_var=relu_var,
-                                scaler_degree=scaler_degree)
+                                scaler_degree=scaler_degree, degree_col=degree_col)
         ctx.save_for_backward(gathered, row_bias, self_feat)
         ctx.meta = (csr, _names(aggregators), _names(scalers), dict(avg_deg), towers, self_divided, messages_in_csr_order,
-                    relu_var, scaler_degree)
+                    relu_var, scaler_degree, degree_col)
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
         gathered, row_bias, self_feat = ctx.saved_tensors
-        csr, aggregators, scalers, avg_deg, towers, self_divided, in_order, relu_var, scaler_degree = ctx.meta
+        csr, aggregators, scalers, avg_deg, towers, self_divided, in_order, relu_var, scaler_degree, degree_col = ctx.meta
         grad_g, grad_b = aggregate_backward(
             grad_out, gathered, csr, aggregators, scalers, avg_deg, towers=towers, row_bias=row_bias,
             has_self=self_feat is not None, messages_in_csr_order=in_order, need_bias_grad=ctx.needs_input_grad[1],
-            relu_var=relu_var, scaler_degree=scaler_degree)
+            relu_var=relu_var, scaler_degree=scaler_degree, degree_col=degree_col)
         gs = None
         if self_feat is not None and ctx.needs_input_grad[2]:
             # the self block of every tower is a plain copy: its gradient is the matching slice of grad_out
@@ -346,14 +362,14 @@ class _PNAAggregate(torch.autograd.Function):
             gs = (blk.reshape(N, F) if self_divided else blk.sum(1)).to(self_feat.dtype)
         return (grad_g.to(gathered.dtype) if ctx.needs_input_grad[0] else None,
                 grad_b.to(row_bias.dtype) if (grad_b is not None) else None, gs,
-                None, None, None, None, None, None, None, None, None, None)
+                None, None, None, None, None, None, None, None, None, None, None)
 
 
 def pna_aggregate(gathered: torch.Tensor, csr: CSRGraph, aggregators: Names, scalers: Names,
                   avg_deg: Mapping[str, float], *, towers: int = 1, row_bias: Optional[torch.Tensor] = None,
                   self_feat: Optional[torch.Tensor] = None, self_divided: bool = True,
                   messages_in_csr_order: bool = False, zero_isolated: bool = False, relu_var: bool = False,
-                  scaler_degree: Optional[torch.Tensor] = None) -> torch.Tensor:
+                  scaler_degree: Optional[torch.Tensor] = None, degree_col: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Differentiable PNA aggregation (forward = one libpna_sm90 call).  See :func:`aggregate_forward`."""
     needs_grad = torch.is_grad_enabled() and any(
         t is not None and t.requires_grad for t in (gathered, row_bias, self_feat))
@@ -361,9 +377,9 @@ def pna_aggregate(gathered: torch.Tensor, csr: CSRGraph, aggregators: Names, sca
         return aggregate_forward(gathered, csr, aggregators, scalers, avg_deg, towers=towers, row_bias=row_bias,
                                  self_feat=self_feat, self_divided=self_divided,
                                  messages_in_csr_order=messages_in_csr_order, zero_isolated=zero_isolated, relu_var=relu_var,
-                                 scaler_degree=scaler_degree)
+                                 scaler_degree=scaler_degree, degree_col=degree_col)
     return _PNAAggregate.apply(gathered, row_bias, self_feat, csr, aggregators, scalers, avg_deg, towers, self_divided,
-                               messages_in_csr_order, zero_isolated, relu_var, scaler_degree)
+                               messages_in_csr_order, zero_isolated, relu_var, scaler_degree, degree_col)
 
 
 def avg_deg_from_histogram(deg: torch.Tensor) -> dict:

@@ -107,8 +107,8 @@ extern "C" int pna_aggregate_fwd(const pna_agg_t* d, pna_stream_t stream) {
     PNA_REQUIRE(((d->scaler_codes >> (4 * s)) & 15u) <= PNA_SCALE_INVERSE_LINEAR, PNA_ERR_BAD_ARG,
                 "pna_aggregate_fwd: bad scaler code");
   PNA_REQUIRE(d->dtype == PNA_F32 || d->dtype == PNA_BF16, PNA_ERR_UNSUPPORTED, "pna_aggregate_fwd: dtype %d", d->dtype);
-  PNA_REQUIRE(!((weighted >> (PNA_AGGR_NORMALISED_MEAN - PNA_AGGR_SOFTMAX)) & 1u) || d->col, PNA_ERR_UNSUPPORTED,
-              "pna_aggregate_fwd: normalised_mean needs col (the source of every slot)");
+  PNA_REQUIRE(!((weighted >> (PNA_AGGR_NORMALISED_MEAN - PNA_AGGR_SOFTMAX)) & 1u) || d->col || d->degree_col,
+              PNA_ERR_UNSUPPORTED, "pna_aggregate_fwd: normalised_mean needs col or degree_col (the source of every slot)");
   if (d->n_rows == 0) return PNA_OK;
   PNA_REQUIRE(d->gathered && d->rowptr && d->out, PNA_ERR_BAD_ARG, "pna_aggregate_fwd: null gathered/rowptr/out");
   PNA_REQUIRE(d->split_threshold >= 2 && d->chunk_edges >= 1, PNA_ERR_BAD_ARG, "pna_aggregate_fwd: bad split/chunk");

@@ -686,8 +686,8 @@ static int bwd_entry(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_o
               "pna_aggregate_bwd_slots");
   PNA_REQUIRE(!weighted || (!d->peer_gathered && !d->row_ids), PNA_ERR_UNSUPPORTED,
               "pna_aggregate_bwd: softmax / softmin / normalised_mean are not available with peer_gathered or row_ids");
-  PNA_REQUIRE(!((weighted >> (PNA_AGGR_NORMALISED_MEAN - PNA_AGGR_SOFTMAX)) & 1u) || d->col, PNA_ERR_UNSUPPORTED,
-              "pna_aggregate_bwd: normalised_mean needs col (the source of every slot)");
+  PNA_REQUIRE(!((weighted >> (PNA_AGGR_NORMALISED_MEAN - PNA_AGGR_SOFTMAX)) & 1u) || d->col || d->degree_col,
+              PNA_ERR_UNSUPPORTED, "pna_aggregate_bwd: normalised_mean needs col or degree_col (the source of every slot)");
   if (d->n_rows == 0) return PNA_OK;
   PNA_REQUIRE(d->gathered && d->rowptr && grad_out && (slots || grad_gathered), PNA_ERR_BAD_ARG, "pna_aggregate_bwd: null pointer");
   PNA_REQUIRE(d->peer_gathered == nullptr, PNA_ERR_UNSUPPORTED, "pna_aggregate_bwd: peer-memory graphs are forward-only");

@@ -67,6 +67,7 @@ struct MParams {
   float* gs; long long ldgs;          // deterministic mode: grad_slots [E, f1 - f0]
   float* gb; long long ldgb;          // grad_row_bias, nullable
   int f0, f1;                         // feature columns handled by this call
+  const int* dcol;                    // normalised_mean: the node whose degree weighs each slot (pna_agg_t.degree_col), or NULL
 };
 
 inline MParams moment_params(const pna_agg_t* d) {
@@ -92,6 +93,7 @@ inline MParams moment_params(const pna_agg_t* d) {
   p.ldeg = (view && d->n_view_rows <= d->n_rows) ? d->light_deg : nullptr;
   p.sdeg = d->scaler_degree;
   p.f0 = 0; p.f1 = d->n_feat;
+  p.dcol = d->degree_col;
   return p;
 }
 

@@ -10,7 +10,8 @@
 // This is the reference's exp(m) / sum exp(m) shifted by the row maximum: equal in exact arithmetic, finite wherever y is
 // (the reference gives inf / inf = NaN above m ~ 88.7).  normalised_mean:
 //   r_k = D_k ? __frsqrt_rn(D_k) : 0,  D_k = rowptr[k+1] - rowptr[k] (the same CSR; D_j = 0 for j >= n_rows),
-//   w_s = fl(r_i * r_col[s]),  y = fp32 sum of fl(m_s * w_s) in slot order.
+//   w_s = fl(r_i * r_j),  j = degree_col[s] when given (messages in CSR order), else col[s],
+//   y = fp32 sum of fl(m_s * w_s) in slot order.
 // y is scaled by the row's scaler factors and stored in its column slot like every other aggregator.  Gradient, with
 // G = sum over the list positions of this aggregator and over the scalers of  scale * grad_out  (positions, then scalers,
 // in order), y' = S / Z:
@@ -77,6 +78,11 @@ __device__ __forceinline__ float wsum_rsqrt_deg(const MParams& p, long long k) {
   return D > 0 ? wsum_rsqrt((float)D) : 0.f;
 }
 
+// the node whose degree weighs slot e: pna_agg_t.degree_col when given, else the slot's source
+__device__ __forceinline__ long long wsum_degree_node(const MParams& p, int e) {
+  return p.dcol ? __ldg(p.dcol + e) : __ldg(p.col + e);
+}
+
 __device__ __forceinline__ float wsum_sigma(unsigned code) { return code == PNA_AGGR_SOFTMIN ? -1.f : 1.f; }
 
 // max over slots [beg, end) of sigma * m
@@ -107,7 +113,7 @@ template <typename T>
 __device__ __forceinline__ float wsum_nmean(const MParams& p, int beg, int end, int f, float b, bool hb, float ri) {
   float s = 0.f;
   for (int e = beg; e < end; ++e) {
-    const float w = __fmul_rn(ri, wsum_rsqrt_deg(p, __ldg(p.col + e)));
+    const float w = __fmul_rn(ri, wsum_rsqrt_deg(p, wsum_degree_node(p, e)));
     s = __fadd_rn(s, __fmul_rn(mom_msg<T>(p, e, f, b, hb), w));
   }
   return s;
@@ -248,7 +254,7 @@ __device__ __forceinline__ float wsum_emit(const MParams& p, int beg, int end, i
   for (int e = beg; e < end; ++e) {
     float g;
     if (code == PNA_AGGR_NORMALISED_MEAN) {
-      g = __fmul_rn(c.a, __fmul_rn(c.ri, wsum_rsqrt_deg(p, __ldg(p.col + e))));
+      g = __fmul_rn(c.a, __fmul_rn(c.ri, wsum_rsqrt_deg(p, wsum_degree_node(p, e))));
     } else {
       const float n = sigma * mom_msg<T>(p, e, f, b, hb);
       const float ex = expf(__fsub_rn(n, c.M));

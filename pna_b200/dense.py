@@ -29,6 +29,13 @@ once).  Where they deliberately differ from the reference:
     isolated node makes the reference's every row NaN (inf * 0 in its diagonal matmul), here that node just has weight 0.
 ``identity`` is X_ii = pretrans([h_i, h_i]) whatever adj says: no kernel call, its column slots are filled here (both
 paths, autograd for its gradient) with the kernels' scaler factors of the loop-free row degree.
+
+``pretrans_layers = L >= 2`` (a ReLU between the layers, so the message is no longer affine): the first layer still
+splits into the node GEMMs A, Bm, b1, and ``pna_edge_mlp_fwd`` (edge_mlp.py) evaluates the rest of the chain once per
+edge of the row CSR, writing M [E, T*F_t] in slot order.  The self-first aggregators read M in CSR order (normalised_mean
+with ``degree_col = row.col``); max/min read the same messages through a third CSR (destination j, sources = the row-slot
+ids of the edges (i, j)), because X[u, v] of the colwise reduction is the message of edge (u, v); ``identity`` runs the
+pretrans MLP on [h_i, h_i] in torch.  Tower widths above 64 raise NotImplementedError.
 """
 from __future__ import annotations
 
@@ -37,6 +44,8 @@ import torch.nn as nn
 
 from .aggregate import aggregate_forward, pna_aggregate
 from .csr import build_csr, tensor_version
+from .edge_mlp import edge_mlp
+from . import _lib
 from .nn_blocks import FCLayer, MLP
 
 _SELF_FIRST = ("mean", "std", "sum", "var", "moment3", "moment4", "moment5", "softmax", "softmin", "normalised_mean")
@@ -60,6 +69,17 @@ class DenseGraphs:
         self.scaler_degree = (adj != 0).sum(-1).reshape(B * N).to(torch.int32).contiguous()
         self.row = build_csr(j + off, i + off, B * N)        # destination i, sources j with adj[i, j] != 0
         self.colwise = build_csr(i + off, j + off, B * N)    # destination j, sources i with adj[i, j] != 0
+        self._pairs = None
+
+    @property
+    def pairs(self):
+        """Destination j, sources = the slot ids of ``row`` whose edge is (i, j) (n_src = E, ascending): the max/min CSR
+        over per-edge messages in row-slot order.  Built on first use (pretrans_layers >= 2 only)."""
+        if self._pairs is None:
+            E, dev = self.row.n_edges, self.row.device
+            self._pairs = build_csr(torch.arange(E, device=dev), self.row.col.long(), self.B * self.N, n_src=E)
+            self._pairs.sources_unique = True       # every slot is the source of exactly one pair
+        return self._pairs
 
 
 _CACHE = {}
@@ -100,6 +120,9 @@ class PNALayer(nn.Module):
         for a in self.aggregators:
             if a not in _SELF_FIRST + _NBR_FIRST + ("identity",):
                 raise KeyError(f"aggregator {a!r} is not available on the CUDA path")
+        if pretrans_layers > 1 and (in_features // towers if divide_input else in_features) > _lib.EDGE_MLP_MAX_WIDTH:
+            raise NotImplementedError(f"dense PNALayer: pretrans_layers > 1 takes a tower input width of at most "
+                                      f"{_lib.EDGE_MLP_MAX_WIDTH} (the edge-MLP kernel's limit)")
         if self_loop and any(a in _MOMENTS for a in self.aggregators):
             raise NotImplementedError("dense PNALayer: moment aggregators with self_loop=True are not supported (the reference "
                                       "centres them on a mean that counts the self loop twice; see the module docstring)")
@@ -144,7 +167,7 @@ class PNALayer(nn.Module):
         h = input.reshape(B * N, Fin)
         T = len(self.towers)
         if not self.towers[0].pretrans.is_single_affine():
-            raise NotImplementedError("dense adapter: pretrans_layers > 1 is not wired to the CUDA path yet")
+            return self._forward_edge_mlp(h, graphs, B, N)
         A, Bm, b = self._halves(h)
         a1 = [a if a in _SELF_FIRST else "_skip" for a in self.aggregators]
         a2 = [a if a in _NBR_FIRST else "_skip" for a in self.aggregators]
@@ -170,6 +193,42 @@ class PNALayer(nn.Module):
             out = torch.where(self._columns(out.size(1), ident, h.device), self._identity_block(A + Bm + b, graphs), out)
         # both calls scale with the ROW degree D = adj.sum(-1) of the loop-free adjacency (scaler_degree), as
         # models/pytorch/pna/scalers.py:13,21 does, whatever edge set the aggregators reduced over
+        out = out.view(B * N, T, -1)
+        y = torch.cat([tw.posttrans(out[:, t]) for t, tw in enumerate(self.towers)], dim=1)
+        return self.mixing_network(y).view(B, N, -1)
+
+    def _forward_edge_mlp(self, h, graphs, B, N):
+        """pretrans_layers >= 2: per-edge messages from pna_edge_mlp_fwd (module docstring), then the same aggregation,
+        scalers, posttrans and mixing as the affine path."""
+        T = len(self.towers)
+        mlps = [tw.pretrans.fully_connected for tw in self.towers]
+        for fcs in mlps:
+            if any(fc.dropout is not None or fc.b_norm is not None for fc in fcs) or \
+                    any(not isinstance(fc.activation, nn.ReLU) for fc in fcs[:-1]) or fcs[-1].activation is not None:
+                raise NotImplementedError("dense PNALayer: the edge-MLP kernel takes Linear/ReLU pretrans layers only")
+        A, Bm, b1 = self._halves(h)
+        W = torch.stack([torch.stack([fcs[k].linear.weight for fcs in mlps]) for k in range(1, len(mlps[0]))])
+        bW = torch.stack([torch.stack([fcs[k].linear.bias for fcs in mlps]) for k in range(1, len(mlps[0]))])
+        M = edge_mlp(A, Bm, b1, W, bW, graphs.row, T)
+        a1 = [a if a in _SELF_FIRST else "_skip" for a in self.aggregators]
+        a2 = [a if a in _NBR_FIRST else "_skip" for a in self.aggregators]
+        common = dict(towers=T, self_feat=h, self_divided=self.divide_input, relu_var=True,
+                      scaler_degree=graphs.scaler_degree)
+        # self first: row i reads the messages of its own slots; normalised_mean weighs slot s with D of col[s]
+        dcol = graphs.row.col if "normalised_mean" in self.aggregators else None
+        out = pna_aggregate(M, graphs.row, a1, self.scalers, self.avg_d, messages_in_csr_order=True, degree_col=dcol,
+                            **common)
+        if any(a != "_skip" for a in a2):
+            # neighbour first: node v reduces X[u, v] = M[slot of edge (u, v)] over u
+            out2 = pna_aggregate(M, graphs.pairs, a2, self.scalers, self.avg_d, **common)
+            both = any(a != "_skip" for a in a1)
+            out = torch.where(self._columns(out.size(1), a2, h.device), out2, out) if both else out2
+        if "identity" in self.aggregators:
+            it = self.input_tower
+            xs = [h[:, t * it:(t + 1) * it] if self.divide_input else h for t in range(T)]
+            x_id = torch.cat([tw.pretrans(torch.cat([x, x], 1)) for x, tw in zip(xs, self.towers)], 1)
+            ident = [a if a == "identity" else "_skip" for a in self.aggregators]
+            out = torch.where(self._columns(out.size(1), ident, h.device), self._identity_block(x_id, graphs), out)
         out = out.view(B * N, T, -1)
         y = torch.cat([tw.posttrans(out[:, t]) for t, tw in enumerate(self.towers)], dim=1)
         return self.mixing_network(y).view(B, N, -1)

@@ -1,0 +1,105 @@
+"""The per-edge pretrans MLP of the dense layer with ``pretrans_layers = L >= 2`` (reference ``models/layers.py:200-229``)
+as one libpna_sm90 call per direction: ``pna_edge_mlp_fwd`` / ``pna_edge_mlp_bwd``.
+
+With one pretrans layer the message is affine and the dense layer gathers two node-level GEMMs.  With L >= 2 a ReLU sits
+between the layers, so the message ``pretrans_t([h_i, h_j])`` has to be evaluated per edge.  The first layer still splits
+into node GEMMs (``A = h W1[:, :F]^T``, ``Bm = h W1[:, F:]^T``); the kernel runs the rest of the chain in registers and
+writes every message once, in CSR slot order.
+
+Backward: the kernel stores the pre-activation gradient of every layer per slot (no atomics); the weight and bias
+gradients are library GEMMs and sums (as ``linear.library_grad_weight``), and ``dA`` / ``dBm`` are the aggregation's
+``sum`` over the row CSR and over its slot-transposed CSR -- fixed orders, so the whole backward is deterministic.
+"""
+from __future__ import annotations
+
+import torch
+
+from . import _lib
+from .aggregate import aggregate_forward
+from .csr import CSRGraph
+
+_ID = {"log": 1.0, "lin": 1.0}
+
+
+def _ptr(t):
+    return None if t is None else t.data_ptr()
+
+
+def _check(A, Bm, b1, W, bW, csr: CSRGraph, towers: int):
+    L1, T, Ft, Ft2 = W.shape
+    if T != towers or Ft != Ft2 or tuple(bW.shape) != (L1, T, Ft) or L1 < 1:
+        raise ValueError(f"edge MLP weights must be [L-1, towers, F_t, F_t] and [L-1, towers, F_t], got {tuple(W.shape)}, "
+                         f"{tuple(bW.shape)}")
+    TF = T * Ft
+    if A.shape != (csr.n_nodes, TF) or Bm.dim() != 2 or Bm.size(1) != TF or tuple(b1.shape) != (TF,):
+        raise ValueError(f"edge MLP inputs must be A [{csr.n_nodes}, {TF}], Bm [n_src, {TF}], b1 [{TF}]")
+    for t in (A, Bm, b1, W, bW):
+        if t.dtype != torch.float32 or not t.is_cuda:
+            raise TypeError("the edge MLP kernel takes float32 CUDA tensors")
+    if Ft > _lib.EDGE_MLP_MAX_WIDTH:
+        raise NotImplementedError(f"edge MLP: tower width {Ft} > {_lib.EDGE_MLP_MAX_WIDTH} is not supported by pna_edge_mlp_fwd")
+    return L1 + 1, T, Ft
+
+
+def edge_mlp_forward(A, Bm, b1, W, bW, csr: CSRGraph, towers: int, store_activations: bool = False):
+    """Messages ``M [E, T*F_t]`` in CSR slot order (and the activations ``[L-1, E, T*F_t]`` when asked)."""
+    L, T, Ft = _check(A, Bm, b1, W, bW, csr, towers)
+    A, Bm, b1, W, bW = (t.contiguous() for t in (A, Bm, b1, W, bW))
+    E, dev = csr.n_edges, A.device
+    M = torch.empty((E, T * Ft), dtype=torch.float32, device=dev)
+    act = torch.empty((L - 1, E, T * Ft), dtype=torch.float32, device=dev) if store_activations else None
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().pna_edge_mlp_fwd(
+            _ptr(csr.rowptr), _ptr(csr.col) if E else None, csr.n_nodes, E, _ptr(A), _ptr(Bm), _ptr(b1), _ptr(W), _ptr(bW),
+            L, T, Ft, _ptr(M), _ptr(act), torch.cuda.current_stream(dev).cuda_stream))
+    return M, act
+
+
+def edge_mlp_backward(grad_M, act, W, n_layers: int, towers: int, width: int):
+    """``[L-1, E, T*F_t]``: the per-slot pre-activation gradients G_1 .. G_(L-1) (G_L is ``grad_M``)."""
+    grad_M, W = grad_M.contiguous().float(), W.contiguous()
+    E, dev = grad_M.size(0), grad_M.device
+    G = torch.empty((n_layers - 1, E, towers * width), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().pna_edge_mlp_bwd(_ptr(grad_M), _ptr(act), _ptr(W), E, n_layers, towers, width, _ptr(G),
+                                               torch.cuda.current_stream(dev).cuda_stream))
+    return G
+
+
+class _EdgeMLP(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, A, Bm, b1, W, bW, csr, towers):
+        M, act = edge_mlp_forward(A, Bm, b1, W, bW, csr, towers, store_activations=True)
+        ctx.save_for_backward(W, act)
+        ctx.meta = (csr, towers, Bm.size(0))
+        return M
+
+    @staticmethod
+    def backward(ctx, grad_M):
+        W, act = ctx.saved_tensors
+        csr, T, n_src = ctx.meta
+        L, Ft = W.size(0) + 1, W.size(2)
+        E = grad_M.size(0)
+        G = edge_mlp_backward(grad_M, act, W, L, T, Ft)
+        grads = [G[k] for k in range(L - 1)] + [grad_M.float()]      # G_1 .. G_L
+        per_tower = lambda x: x.reshape(E, T, Ft)
+        # layer k = 2..L: dW_k[t] = G_k[:, t]^T z_(k-1)[:, t],  db_k[t] = sum over slots of G_k[:, t]
+        dW = torch.stack([torch.bmm(per_tower(grads[k - 1]).permute(1, 2, 0), per_tower(act[k - 2]).permute(1, 0, 2))
+                          for k in range(2, L + 1)])
+        dbW = torch.stack([per_tower(grads[k - 1]).sum(0) for k in range(2, L + 1)])
+        G1 = grads[0]
+        dA = dBm = None
+        if ctx.needs_input_grad[0]:     # sum of G_1 over the slots of every row (slot order)
+            dA = aggregate_forward(G1, csr, ["sum"], ["identity"], _ID, messages_in_csr_order=True)
+        if ctx.needs_input_grad[1]:     # sum of G_1 over the out-edges of every source (ascending slot ids)
+            dBm = aggregate_forward(G1, csr.slot_transposed(n_src), ["sum"], ["identity"], _ID)
+        db1 = G1.sum(0)
+        return dA, dBm, db1, dW, dbW, None, None
+
+
+def edge_mlp(A, Bm, b1, W, bW, csr: CSRGraph, towers: int) -> torch.Tensor:
+    """Differentiable per-edge MLP messages ``[E, T*F_t]`` in slot order of ``csr``:
+    ``M[s, t] = W_L[t] relu(... relu(A[i, t] + Bm[col[s], t] + b1[t]) ...) + b_L[t]`` (see include/pna_b200.h)."""
+    if torch.is_grad_enabled() and any(t.requires_grad for t in (A, Bm, b1, W, bW)):
+        return _EdgeMLP.apply(A, Bm, b1, W, bW, csr, towers)
+    return edge_mlp_forward(A, Bm, b1, W, bW, csr, towers)[0]
