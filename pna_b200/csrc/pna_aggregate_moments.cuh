@@ -1,7 +1,7 @@
 // The moment3 / moment4 / moment5 aggregators (reference models/pytorch/pna/aggregators.py:122-146), forward and backward.
 //
 // For destination row i with messages m_s (row_bias added when given), d = |In(i)| and k in {3, 4, 5}:
-//   mu    = fp32 sum of m_s in slot order, divided by d (SharedDivisor: the correctly rounded quotient, as for `mean`)
+//   mu    = fp32 sum of m_s in slot order, divided by d (mom_div: the correctly rounded quotient)
 //   delta = fl(m_s - mu);  delta^2 = fl(delta * delta), delta^(j+1) = fl(delta^j * delta)   (one rounding per product)
 //   M_k   = (fp32 sum of delta^k in slot order) / d          (correctly rounded)
 //   r_k   = sign(M_k) * (|M_k| + 1e-5)^(1/k)                 (powf, exponent 1/k rounded to fp32);  d == 0: r_k = 0
@@ -146,6 +146,11 @@ __device__ __forceinline__ Pow4 mom_central(const MParams& p, int beg, int end, 
   return acc;
 }
 
+// x / d correctly rounded (IEEE division).  Not SharedDivisor: its reciprocal-and-correction sequence gives NaN for an
+// infinite numerator (a sum of overflowed powers, inf - inf in the correction) and may miss a subnormal quotient by one
+// ulp; these kernels divide a handful of times per row, so the full division costs nothing measurable.
+__device__ __forceinline__ float mom_div(float x, int d) { return __fdiv_rn(x, (float)d); }
+
 __device__ __forceinline__ float moment_inv(int k) { return k == 3 ? (1.0f / 3.0f) : k == 4 ? 0.25f : 0.2f; }
 
 // sign(M) * (|M| + 1e-5)^(1/k); 0 (and NaN) pass through
@@ -210,11 +215,10 @@ __global__ void __launch_bounds__(kMomThreads) k_mom_rows(const MParams p) {
   if (deg > 0) {
     const bool hb = p.bias != nullptr;
     const float b = mom_bias<T>(p, row, f);
-    const SharedDivisor by_d((float)deg);
-    const float mu = by_d(mom_sum<T>(p, beg, end, f, b, hb));
+    const float mu = mom_div(mom_sum<T>(p, beg, end, f, b, hb), deg);
     const Pow4 c = mom_central<T>(p, beg, end, f, b, hb, mu);
 #pragma unroll
-    for (int j = 0; j < 3; ++j) M[j] = by_d(c.q[j + 1]);
+    for (int j = 0; j < 3; ++j) M[j] = mom_div(c.q[j + 1], deg);
   }
   mom_store<T>(p, row, deg, f, M);
 }
@@ -255,7 +259,7 @@ __global__ void __launch_bounds__(kMomThreads) k_mom_hub_mean(const MParams p) {
   const int first = __ldg(p.hub_info + 4 * h + 1), nch = __ldg(p.hub_info + 4 * h + 2), deg = __ldg(p.hub_info + 4 * h + 3);
   float s = 0.f;
   for (int j = 0; j < nch; ++j) s = __fadd_rn(s, *mom_part<W>(p, first + j, 0, f));
-  const float mu = SharedDivisor((float)deg)(s);
+  const float mu = mom_div(s, deg);
   if (W == 4) *mom_part<W>(p, first, 1, f) = mu;
   else *mom_part<W>(p, p.n_chunks + h, 0, f) = mu;
 }
@@ -291,8 +295,7 @@ __global__ void __launch_bounds__(kMomThreads) k_mom_hub_final(const MParams p) 
     s4 = __fadd_rn(s4, *mom_part<4>(p, first + j, 2, f));
     s5 = __fadd_rn(s5, *mom_part<4>(p, first + j, 3, f));
   }
-  const SharedDivisor by_d((float)deg);
-  const float M[3] = {by_d(s3), by_d(s4), by_d(s5)};
+  const float M[3] = {mom_div(s3, deg), mom_div(s4, deg), mom_div(s5, deg)};
   mom_store<T>(p, row, deg, f, M);
 }
 
@@ -314,12 +317,11 @@ __device__ __forceinline__ MomCoef mom_coef(const MParams& p, long long row, int
       G[k - 3] = __fadd_rn(G[k - 3], sc == PNA_SCALE_IDENTITY ? go : __fmul_rn(ds.of(sc), go));
     }
   }
-  const SharedDivisor by_d((float)deg);
   float a[3], C[3];
   for (int i = 0; i < 3; ++i) {
     const int k = i + 3;
-    C[i] = by_d(P.q[i]);                                   // C_(k-1)
-    a[i] = (p.orders >> i) & 1u ? __fmul_rn(__fmul_rn(G[i], moment_slope(by_d(P.q[i + 1]), k)), by_d((float)k)) : 0.f;
+    C[i] = mom_div(P.q[i], deg);                           // C_(k-1)
+    a[i] = (p.orders >> i) & 1u ? __fmul_rn(__fmul_rn(G[i], moment_slope(mom_div(P.q[i + 1], deg), k)), mom_div((float)k, deg)) : 0.f;
   }
   MomCoef c;
   c.a3 = a[0]; c.a4 = a[1]; c.a5 = a[2];
@@ -371,7 +373,7 @@ __global__ void __launch_bounds__(kMomThreads) k_mom_bwd_rows(const MParams p) {
   if (deg == 0 || deg >= p.split) return;
   const bool hb = p.bias != nullptr;
   const float b = mom_bias<T>(p, row, f);
-  const float mu = SharedDivisor((float)deg)(mom_sum<T>(p, beg, end, f, b, hb));
+  const float mu = mom_div(mom_sum<T>(p, beg, end, f, b, hb), deg);
   const MomCoef c = mom_coef<T>(p, row, deg, f, mom_central<T>(p, beg, end, f, b, hb, mu));
   const float gbs = mom_emit<T, SLOTS>(p, beg, end, f, b, hb, mu, c);
   if (p.gb) {
