@@ -70,6 +70,15 @@ __device__ __forceinline__ float lin_tf32(float x) {
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
   return __uint_as_float(r);
 }
+// the hi part: cvt.rna rounds every finite |x| >= 0x7F7FF000 (within 2^-11 of FLT_MAX) up to inf, and x - hi would then
+// be -inf (the product NaN); satfinite clamps hi to the largest TF32 value instead, so lo = x - hi stays exact and finite.
+// An inf input gets hi = +-MAX and lo = +-inf (plain cvt.rna keeps lo infinite): the products give what fp32 gives.
+__device__ __forceinline__ void lin_split(float x, float& hi, float& lo) {
+  unsigned r;
+  asm("cvt.rna.satfinite.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+  hi = __uint_as_float(r);
+  lo = lin_tf32(x - hi);
+}
 
 // wgmma shared-memory matrix descriptor: K-major, SWIZZLE_128B, rows of 128 bytes, 8-row groups 1024 bytes apart.
 // A K step inside the 128-byte row advances the start address (the swizzle is applied to the computed addresses).
@@ -266,10 +275,10 @@ k_linear_3xtf32(const float* __restrict__ A, long long lda, const float* __restr
               v.z = __fmul_rn(v.z, sc[sl]); v.w = __fmul_rn(v.w, sc[sl]);
             }
             float4 hi, lo;
-            hi.x = lin_tf32(v.x); lo.x = lin_tf32(v.x - hi.x);
-            hi.y = lin_tf32(v.y); lo.y = lin_tf32(v.y - hi.y);
-            hi.z = lin_tf32(v.z); lo.z = lin_tf32(v.z - hi.z);
-            hi.w = lin_tf32(v.w); lo.w = lin_tf32(v.w - hi.w);
+            lin_split(v.x, hi.x, lo.x);
+            lin_split(v.y, hi.y, lo.y);
+            lin_split(v.z, hi.z, lo.z);
+            lin_split(v.w, hi.w, lo.w);
             const unsigned off = lin_swz(sl * 32 + r_in, j);  // quarter-warps write whole swizzled 128-byte rows: conflict free
             *reinterpret_cast<float4*>(st + off) = hi;
             *reinterpret_cast<float4*>(st + LinSmem<O>::kATile + off) = lo;
@@ -333,10 +342,10 @@ __global__ void k_split_weight(const float* __restrict__ W, int O, int K, float*
   const int kb = u / 8, j = u % 8;
   const float4 w = *reinterpret_cast<const float4*>(W + (long long)r * K + u * 4);
   float4 hi, lo;
-  hi.x = lin_tf32(w.x); lo.x = lin_tf32(w.x - hi.x);
-  hi.y = lin_tf32(w.y); lo.y = lin_tf32(w.y - hi.y);
-  hi.z = lin_tf32(w.z); lo.z = lin_tf32(w.z - hi.z);
-  hi.w = lin_tf32(w.w); lo.w = lin_tf32(w.w - hi.w);
+  lin_split(w.x, hi.x, lo.x);
+  lin_split(w.y, hi.y, lo.y);
+  lin_split(w.z, hi.z, lo.z);
+  lin_split(w.w, hi.w, lo.w);
   float* tile = img + (long long)kb * (2 * O * kLinBK);
   const unsigned off = lin_swz(r, j) / 4;
   *reinterpret_cast<float4*>(tile + off) = hi;
@@ -385,10 +394,10 @@ __global__ void k_split_weight_t(const float* __restrict__ W, int O, int n_in, i
 #pragma unroll
   for (int e = 0; e < 4; ++e) v[e] = c < n_cols ? __ldg(W + (long long)(o + e) * n_in + s * n_cols + c) : 0.f;
   float4 hi, lo;
-  hi.x = lin_tf32(v[0]); lo.x = lin_tf32(v[0] - hi.x);
-  hi.y = lin_tf32(v[1]); lo.y = lin_tf32(v[1] - hi.y);
-  hi.z = lin_tf32(v[2]); lo.z = lin_tf32(v[2] - hi.z);
-  hi.w = lin_tf32(v[3]); lo.w = lin_tf32(v[3] - hi.w);
+  lin_split(v[0], hi.x, lo.x);
+  lin_split(v[1], hi.y, lo.y);
+  lin_split(v[2], hi.z, lo.z);
+  lin_split(v[3], hi.w, lo.w);
   float* tile = img + ((long long)slab * n_kbw + kbw) * (2 * Os * kLinBK);
   const unsigned off = lin_swz(r, j) / 4;
   *reinterpret_cast<float4*>(tile + off) = hi;
@@ -506,10 +515,10 @@ k_linear_bwd_weight(const float* __restrict__ dY, long long ldy, const float* __
       for (int e = 0; e < 4; ++e) {
         float4 hi, lo;
         const float v0 = lin_comp(src[m][0], e), v1 = lin_comp(src[m][1], e), v2 = lin_comp(src[m][2], e), v3 = lin_comp(src[m][3], e);
-        hi.x = lin_tf32(v0); lo.x = lin_tf32(v0 - hi.x);
-        hi.y = lin_tf32(v1); lo.y = lin_tf32(v1 - hi.y);
-        hi.z = lin_tf32(v2); lo.z = lin_tf32(v2 - hi.z);
-        hi.w = lin_tf32(v3); lo.w = lin_tf32(v3 - hi.w);
+        lin_split(v0, hi.x, lo.x);
+        lin_split(v1, hi.y, lo.y);
+        lin_split(v2, hi.z, lo.z);
+        lin_split(v3, hi.w, lo.w);
         const unsigned off = lin_swz(4 * q + e, jj);
         *reinterpret_cast<float4*>(hi_t + off) = hi;
         *reinterpret_cast<float4*>(lo_t + off) = lo;
