@@ -321,6 +321,24 @@ int pna_edge_mlp_fwd(const int32_t* rowptr, const int32_t* col, int64_t n_rows, 
 int pna_edge_mlp_bwd(const float* grad_messages, const float* activations, const float* weight, int64_t n_edges,
                      int32_t n_layers, int32_t n_towers, int32_t width, float* grad_pre, pna_stream_t stream);
 
+/* ---- per-edge messages of the PyG PNAConv and the DGL PNALayer: the same MLP with an edge term, any L >= 1 ------------
+ * As pna_edge_mlp_fwd, with two changes (rounding order: pna_b200/csrc/pna_edge_mlp.cu):
+ *   u1 = fl(fl(fl(a[i, t] + b[j, t]) + bias1[t]) + edge_term[s, t])      edge_term (nullable) [n_edges, TF], slot order;
+ *                                                                         NULL: exactly pna_edge_mlp_fwd's u1
+ *   messages [n_edges, n_towers * msg_pitch]: messages[s, t*msg_pitch + o] = u_L,o for o < width and exact zeros for
+ *   width <= o < msg_pitch, so the aggregation reads it at width msg_pitch with n_towers towers.
+ * n_layers == 1: the message is u1 itself (no ReLU; weight, bias and activations are not read) and any width is taken.
+ * n_layers >= 2: width <= PNA_EDGE_MLP_MAX_WIDTH; activations (nullable) as pna_edge_mlp_fwd, at pitch width.
+ * pna_edge_msg_bwd (n_layers >= 2): pna_edge_mlp_bwd with grad_messages read at pitch msg_pitch; grad_pre at pitch width.
+ * n_layers < 1 (< 2 for the backward), msg_pitch < width, width < 1, n_towers < 1 or a null required pointer (with
+ * n_edges > 0): PNA_ERR_BAD_ARG; n_layers >= 2 with width > PNA_EDGE_MLP_MAX_WIDTH: PNA_ERR_UNSUPPORTED. */
+int pna_edge_msg_fwd(const int32_t* rowptr, const int32_t* col, int64_t n_rows, int64_t n_edges, const float* a, const float* b,
+                     const float* bias1, const float* edge_term, const float* weight, const float* bias, int32_t n_layers,
+                     int32_t n_towers, int32_t width, int32_t msg_pitch, float* messages, float* activations,
+                     pna_stream_t stream);
+int pna_edge_msg_bwd(const float* grad_messages, int32_t msg_pitch, const float* activations, const float* weight,
+                     int64_t n_edges, int32_t n_layers, int32_t n_towers, int32_t width, float* grad_pre, pna_stream_t stream);
+
 /* ---- halo rows for the destination-partitioned multi-GPU path (north_star: "single NCCL all-to-all for halo
  * source features per layer"): dst[i, :] = src[idx[i], :], n_feat elements per row.  Used to pack the send buffer. */
 int pna_gather_rows(const void* src, int64_t ld_src, const int32_t* idx, int64_t n_idx, void* dst, int64_t ld_dst,

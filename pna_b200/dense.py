@@ -202,10 +202,8 @@ class PNALayer(nn.Module):
         scalers, posttrans and mixing as the affine path."""
         T = len(self.towers)
         mlps = [tw.pretrans.fully_connected for tw in self.towers]
-        for fcs in mlps:
-            if any(fc.dropout is not None or fc.b_norm is not None for fc in fcs) or \
-                    any(not isinstance(fc.activation, nn.ReLU) for fc in fcs[:-1]) or fcs[-1].activation is not None:
-                raise NotImplementedError("dense PNALayer: the edge-MLP kernel takes Linear/ReLU pretrans layers only")
+        if not all(tw.pretrans.is_linear_relu() for tw in self.towers):
+            raise NotImplementedError("dense PNALayer: the edge-MLP kernel takes Linear/ReLU pretrans layers only")
         A, Bm, b1 = self._halves(h)
         W = torch.stack([torch.stack([fcs[k].linear.weight for fcs in mlps]) for k in range(1, len(mlps[0]))])
         bW = torch.stack([torch.stack([fcs[k].linear.bias for fcs in mlps]) for k in range(1, len(mlps[0]))])

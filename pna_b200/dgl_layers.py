@@ -5,6 +5,15 @@ Same constructors, same ``forward(g, h, e, snorm_n)`` / ``forward(g, h)``, same 
 ``mixing_network.linear``; ``posttrans`` / ``batchnorm_h`` for the simple layer).  ``g`` is duck-typed (graph.py).
 DGL's ``apply_edges`` + ``update_all`` with a Python reduce UDF per in-degree bucket (pna_layer.py:61-64,202) is
 replaced by ONE kernel call over all towers; in-degree-0 nodes keep DGL's zero rows (PNA_FLAG_ZERO_ISOLATED).
+
+``PNALayer`` messages (pna_layer.py:35-40, ``pretrans(cat[src h, dst h, ef])``): without edge features and with one
+pretrans layer they are affine and never built (two node GEMMs and the aggregation's row bias).  With edge features or
+``pretrans_layers > 1`` they are written once, in CSR slot order at the padded tower width, by ``pna_edge_msg_fwd``
+(edge_mlp.py): node GEMMs for the source and destination halves of the first pretrans Linear, one GEMM of the permuted
+``ef`` against every tower's edge columns, and the rest of the pretrans MLP per edge.  The towers' ``pretrans`` run in
+torch on gathered rows only for inputs the kernel does not take: dtypes other than float32, ``pretrans_layers > 1`` with
+a tower width above 64, pretrans stacks that are not plain Linear / ReLU (dropout or batch norm inside), and training
+steps on graphs below ``edge_mlp.FUSED_TRAINING_MIN_EDGES`` edges, where the torch path measured faster.
 """
 from __future__ import annotations
 
@@ -12,8 +21,10 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import padding as pad
+from . import _lib, padding as pad
 from .aggregate import pna_aggregate, row_scales
+from . import edge_mlp
+from .edge_mlp import edge_messages
 from .linear import compact_path_ok
 from .csr import tensor_version
 from .graph import graph_csr
@@ -121,6 +132,54 @@ class PNALayer(nn.Module):
         half = uv.size(1) // 2
         return uv[:, :half], uv[:, half:]
 
+    def _fused_messages_ok(self, h, e, n_edges: int) -> bool:
+        """The inputs pna_edge_msg_fwd takes: float32 on the GPU, Linear/ReLU pretrans stacks, and a tower width of at
+        most 64 when there is more than one pretrans layer; with autograd, graphs of at least
+        edge_mlp.FUSED_TRAINING_MIN_EDGES edges (where the kernel path is faster)."""
+        fc0 = self.towers[0].pretrans.fully_connected
+        return (edge_mlp.fused_step_pays(n_edges) and h.is_cuda and h.dtype == torch.float32 and fc0[0].linear.weight.dtype == torch.float32
+                and (not self.edge_features or (e is not None and e.dtype == torch.float32))
+                and all(tw.pretrans.is_linear_relu() for tw in self.towers)
+                and (len(fc0) == 1 or self.input_tower <= _lib.EDGE_MLP_MAX_WIDTH))
+
+    def _fused_messages(self, csr, h, e, fp):
+        """[E, T*fp] messages in slot order from pna_edge_msg_fwd, concatenation order [src h, dst h, ef]: Bm = h W[:, :it]^T
+        (source side), A = h W[:, it:2it]^T (destination side), block-diagonal under divide_input; C = ef[perm] W_e^T with
+        W_e every tower's W[:, 2it:] stacked (ef is not split by divide_input); the hidden Linears as [L-1, T, it, it]."""
+        Wd, Ws, b1, We, W, bW = self._message_weights()
+        C = e.index_select(0, csr.perm.long()) @ We.t() if self.edge_features else None
+        return edge_messages(h @ Wd.t(), h @ Ws.t(), b1, W, bW, csr, len(self.towers), edge_term=C, pitch=fp)
+
+    def _message_weights(self):
+        """The pretrans weights packed as the kernel takes them; rebuilt only when a parameter changed (without autograd;
+        with autograd the pack is part of the graph and rebuilt every call), as ``_affine_terms``."""
+        it = self.input_tower
+        fcs = [tw.pretrans.fully_connected for tw in self.towers]
+        params = [p_ for f in fcs for fc in f for p_ in (fc.linear.weight, fc.linear.bias)]
+        key = (tuple(tensor_version(p_) for p_ in params), tuple(p_.data_ptr() for p_ in params))
+        cache = not (torch.is_grad_enabled() and any(p_.requires_grad for p_ in params))
+        hit = getattr(self, "_msg_pack", None)
+        if cache and hit is not None and hit[0] == key:
+            return hit[1]
+        W1 = [f[0].linear.weight for f in fcs]
+        Ws, Wd = [w[:, :it] for w in W1], [w[:, it:2 * it] for w in W1]
+        if self.divide_input and len(fcs) > 1:
+            Wd, Ws = torch.block_diag(*Wd), torch.block_diag(*Ws)
+        else:
+            Wd, Ws = torch.cat(Wd, 0), torch.cat(Ws, 0)
+        b1 = torch.cat([f[0].linear.bias for f in fcs])
+        We = torch.cat([w[:, 2 * it:] for w in W1], 0) if self.edge_features else None
+        L = len(fcs[0])
+        if L > 1:
+            W = torch.stack([torch.stack([f[k].linear.weight for f in fcs]) for k in range(1, L)])
+            bW = torch.stack([torch.stack([f[k].linear.bias for f in fcs]) for k in range(1, L)])
+        else:
+            W = bW = W1[0].new_empty(0)
+        pack = (Wd, Ws, b1, We, W, bW)
+        if cache:
+            self._msg_pack = (key, pack)
+        return pack
+
     def _edge_messages(self, csr, h, e):
         src, dst = csr.col.long(), csr.dst_of_slot
         ef = e.index_select(0, csr.perm.long()) if self.edge_features else None
@@ -147,7 +206,10 @@ class PNALayer(nn.Module):
             U, V = self._affine_terms(h, fp)
             agg = pna_aggregate(V, csr, self.aggregators, self.scalers, self.avg_d, row_bias=U, **common)
         else:
-            msgs = pad.pad_blocks(self._edge_messages(csr, h, e), T, it, fp)
+            if self._fused_messages_ok(h, e, csr.n_edges):
+                msgs = self._fused_messages(csr, h, e, fp)
+            else:
+                msgs = pad.pad_blocks(self._edge_messages(csr, h, e), T, it, fp)
             agg = pna_aggregate(msgs, csr, self.aggregators, self.scalers, self.avg_d, messages_in_csr_order=True, **common)
         agg = agg.view(h.size(0), T, -1)                                  # [N, T, (1 + S*A) * fp] = cat([h_t, reduced])
         blocks = 1 + len(self.aggregators) * len(self.scalers)

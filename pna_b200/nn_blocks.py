@@ -93,5 +93,12 @@ class MLP(nn.Module):
         fc = self.fully_connected[0]
         return len(self.fully_connected) == 1 and fc.activation is None and fc.dropout is None and fc.b_norm is None
 
+    def is_linear_relu(self) -> bool:
+        """True when every layer is a bare Linear with a ReLU between layers and none after the last: the stack the
+        per-edge message kernels (edge_mlp.py) evaluate."""
+        fcs = self.fully_connected
+        return not any(fc.dropout is not None or fc.b_norm is not None for fc in fcs) and \
+            all(isinstance(fc.activation, nn.ReLU) for fc in fcs[:-1]) and fcs[-1].activation is None
+
     def __repr__(self):
         return f"{self.__class__.__name__} ({self.in_size} -> {self.out_size})"

@@ -13,8 +13,10 @@ import torch
 from torch import Tensor
 from torch.nn import Linear, Module, ModuleList, ReLU, Sequential
 
-from . import padding as pad
+from . import _lib, padding as pad
 from .aggregate import avg_deg_from_histogram, pna_aggregate, row_scales
+from . import edge_mlp
+from .edge_mlp import edge_messages
 from .linear import compact_path_ok, linear_tf32x3, post_linear, post_linear_scaled
 from .csr import CSRGraph, csr_from_edge_index, tensor_version
 
@@ -162,7 +164,13 @@ class PNAConv(Module):
     With ``pre_layers == 1`` and no edge features the message is affine in (x_i, x_j):
     ``m = W_i x_i + W_j x_j + b`` (pna.py:94,147-149), so the E x F message tensor is never built: two node-level
     GEMMs give ``U = x W_i^T`` and ``V = x W_j^T + b`` and the kernel gathers V and adds U[i] per slot.  Otherwise
-    the messages are materialised in CSR slot order and reduced by the same kernel.
+    (edge features or ``pre_layers > 1``) the messages are written once, in CSR slot order at the padded tower width, by
+    ``pna_edge_msg_fwd`` (edge_mlp.py): the first pre Linear splits into the node GEMMs ``A = x W_i^T``,
+    ``Bm = x W_j^T`` and one edge GEMM ``C = edge_encoder(edge_attr)[perm] W_e^T`` for all towers, and the kernel runs
+    the rest of the pre-MLP per edge; the aggregation then reads them in slot order.  The messages are built in torch
+    (the towers' ``pre_nns`` on gathered rows) only for inputs the kernel does not take: dtypes other than float32, and
+    ``pre_layers > 1`` with a tower width ``F_in`` above 64 -- and for training steps on graphs below
+    ``edge_mlp.FUSED_TRAINING_MIN_EDGES`` edges, where the torch path measured faster (launch overhead).
     """
 
     def __init__(self, in_channels: int, out_channels: int, aggregators: List[str], scalers: List[str], deg: Tensor,
@@ -250,6 +258,50 @@ class PNAConv(Module):
         uv = torch.addmm(b_uv, x, w_uv.t())
         h = uv.size(1) // 2
         return uv[:, :h], uv[:, h:]
+
+    def _fused_messages_ok(self, x: Tensor, edge_attr: Optional[Tensor], n_edges: int) -> bool:
+        """The inputs pna_edge_msg_fwd takes: float32 on the GPU, and a tower width of at most 64 with pre_layers > 1;
+        with autograd, graphs of at least edge_mlp.FUSED_TRAINING_MIN_EDGES edges (where the kernel path is faster)."""
+        return (edge_mlp.fused_step_pays(n_edges) and x.is_cuda and x.dtype == torch.float32 and self.pre_nns[0][0].weight.dtype == torch.float32
+                and (edge_attr is None) == (self.edge_dim is None)
+                and (self.pre_layers == 1 or self.F_in <= _lib.EDGE_MLP_MAX_WIDTH))
+
+    def _fused_messages(self, x: Tensor, csr: CSRGraph, edge_attr: Optional[Tensor], Fp: int) -> Tensor:
+        """[E, T*Fp] messages in slot order from pna_edge_msg_fwd: A = x W_i^T (x_i side), Bm = x W_j^T (x_j side),
+        block-diagonal under divide_input; C = edge_encoder(edge_attr)[perm] W_e^T with W_e the towers' W[:, 2F:3F]
+        stacked (one GEMM); the hidden Linears stacked as [L-1, T, F, F]."""
+        Wi, Wj, b1, We, W, bW = self._message_weights()
+        C = None
+        if edge_attr is not None:
+            C = self.edge_encoder(edge_attr).index_select(0, csr.perm.long()) @ We.t()
+        return edge_messages(x @ Wi.t(), x @ Wj.t(), b1, W, bW, csr, self.towers, edge_term=C, pitch=Fp)
+
+    def _message_weights(self):
+        """The pre_nns weights packed as the kernel takes them, cached per parameter version like ``_prepared``."""
+        T, Fi = self.towers, self.F_in
+        lins = [list(nn)[0::2] for nn in self.pre_nns]           # the Linears of each tower (ReLU between them)
+        params = [p_ for l in lins for lin in l for p_ in lin.parameters()]
+        key = (tuple(tensor_version(p_) for p_ in params), tuple(p_.data_ptr() for p_ in params))
+        cache = torch.is_grad_enabled() is False or not any(p_.requires_grad for p_ in params)
+        if cache and getattr(self, "_msg_pack", None) is not None and self._msg_pack[0] == key:
+            return self._msg_pack[1]
+        W1 = [l[0].weight for l in lins]
+        Wi, Wj = [w[:, :Fi] for w in W1], [w[:, Fi:2 * Fi] for w in W1]
+        if self.divide_input and T > 1:
+            Wi, Wj = torch.block_diag(*Wi), torch.block_diag(*Wj)
+        else:
+            Wi, Wj = torch.cat(Wi, 0), torch.cat(Wj, 0)
+        b1 = torch.cat([l[0].bias for l in lins])
+        We = torch.cat([w[:, 2 * Fi:3 * Fi] for w in W1], 0) if self.edge_dim is not None else None
+        if self.pre_layers > 1:
+            W = torch.stack([torch.stack([l[k].weight for l in lins]) for k in range(1, self.pre_layers)])
+            bW = torch.stack([torch.stack([l[k].bias for l in lins]) for k in range(1, self.pre_layers)])
+        else:
+            W = bW = W1[0].new_empty(0)
+        pack = (Wi, Wj, b1, We, W, bW)
+        if cache:
+            self._msg_pack = (key, pack)
+        return pack
 
     def _messages_in_slot_order(self, x: Tensor, csr: CSRGraph, edge_attr: Optional[Tensor]) -> Tensor:
         """General path (edge features or pre_layers > 1): pna.py:137-150 evaluated on CSR-ordered edges."""
@@ -346,7 +398,10 @@ class PNAConv(Module):
             U, V = self._affine_terms(x, Fp)
             out = pna_aggregate(V, csr, self.aggregators, self.scalers, self.avg_deg, row_bias=U, **common)
         else:
-            msgs = pad.pad_blocks(self._messages_in_slot_order(x, csr, edge_attr), T, Fi, Fp)
+            if self._fused_messages_ok(x, edge_attr, csr.n_edges):
+                msgs = self._fused_messages(x, csr, edge_attr, Fp)
+            else:
+                msgs = pad.pad_blocks(self._messages_in_slot_order(x, csr, edge_attr), T, Fi, Fp)
             out = pna_aggregate(msgs, csr, self.aggregators, self.scalers, self.avg_deg, messages_in_csr_order=True,
                                 **common)
         out = out.view(x.size(0), T, -1)                       # [N, T, (1 + S*A) * Fp]  (pna.py:131)
