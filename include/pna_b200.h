@@ -428,6 +428,28 @@ int pna_linear_bwd_weight(const float* grad_y, int64_t ld_grad_y, const float* a
 int pna_row_scales(const int32_t* rowptr, int64_t n_rows, int32_t n_scalers, uint32_t scaler_codes, float avg_log, float avg_lin,
                    float* scales, pna_stream_t stream);
 
+/* ---- first post Linear of the tower layers (PNAConv, the DGL PNALayer) on the compact tower aggregate (3xTF32) ----------
+ * a [n_rows, T * (1 + A) * F] (pitch lda) is what pna_aggregate_fwd writes with self_feat and the identity scaler alone:
+ * per tower t the block [self_t | agg_t] of F + A * F columns.  weight [T, n_out, (1 + S * A) * F] contiguous is every
+ * tower's first post Linear in the reference's column layout (self block, then scaler-major aggregate blocks), bias
+ * [T, n_out] or NULL, row_scale the [n_rows, S] factors of pna_row_scales.  y [n_rows, T * n_out] (pitch ldy), tower-major:
+ *     y[i, t * n_out + o] = b_t[o] + sum_k self_t[i, k] W_t[o, k] + sum_s sum_k fl(row_scale[i, s] * agg_t[i, k]) W_t[o, F + s A F + k]
+ * Each tower reads only its own columns; the scaled copies exist only in registers.  Same split and fp32 accuracy as
+ * pna_linear_fwd; the tensor-core chains are folded into an fp32 total every 128 products.
+ * pna_linear_towers_bwd_data writes grad_a [n_rows, T * (1 + A) * F] (pitch ld_grad_a) from grad_y [n_rows, T * n_out]:
+ *     self columns       grad_a[i, t, k]     = sum_o grad_y[i, t, o] W_t[o, k]
+ *     aggregate columns  grad_a[i, t, F + k] = sum_s sum_o fl(row_scale[i, s] * grad_y[i, t, o]) W_t[o, F + s A F + k]
+ * with the same folds.  Neither call uses atomics or a workspace; the results are a fixed function of the inputs.
+ * n_towers <= 8, n_out <= 64, n_towers * n_out <= 256 and F % 4 == 0, else PNA_ERR_UNSUPPORTED; n_scalers outside 1..5,
+ * n_aggr outside 1..6, a null pointer or a pitch shorter than the row: PNA_ERR_BAD_ARG.  No alignment is required.
+ * n_rows == 0 returns PNA_OK and launches nothing.  (Appended in ABI version 8.) */
+int pna_linear_towers_scaled_fwd(const float* a, int64_t lda, const float* row_scale, int32_t n_scalers, const float* weight,
+                                 const float* bias, float* y, int64_t ldy, int64_t n_rows, int32_t n_towers, int32_t n_feat,
+                                 int32_t n_aggr, int32_t n_out, pna_stream_t stream);
+int pna_linear_towers_bwd_data(const float* grad_y, int64_t ld_grad_y, const float* row_scale, int32_t n_scalers, const float* weight,
+                               float* grad_a, int64_t ld_grad_a, int64_t n_rows, int32_t n_towers, int32_t n_feat, int32_t n_aggr,
+                               int32_t n_out, pna_stream_t stream);
+
 int pna_query(int what);
 const char* pna_last_error(void);
 

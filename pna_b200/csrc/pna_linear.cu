@@ -627,6 +627,202 @@ static int launch_bwd_weight(const float* dY, long long ldy, const float* A, lon
   return PNA_OK;
 }
 
+// ============================ tower post linear (pna_linear_towers_scaled_fwd / pna_linear_towers_bwd_data) ============================
+//
+// PNAConv / the DGL PNALayer with T towers: tower t's first post Linear reads [self_t | cat_s(c_s(i) * agg_t)] (pna.py:131-132,
+// pna_layer.py:67).  The aggregation writes the COMPACT per-tower block [self_t | agg_t] ((1 + A) * Fp columns, identity scaler
+// only) and the loaders form every scaled copy in registers, as pna_linear_scaled_fwd does for one tower.  Each CTA computes a
+// 128-row x 64-column tile of ONE tower's output from that tower's own columns only (no block-diagonal zero work).
+//
+// A tower's operand is a VIRTUAL K axis that the loaders gather column by column:
+//     k < L0:               x[i, k]                                          (forward: the self block; data gradient: dY_t)
+//     k = L0 + s * L1 + q:  fl(c_s(i) * x[i, c1 + q])   s < S, q < L1          (forward: agg_t; data gradient: dY_t again)
+//     k >= L0 + S * L1:     0                                                 (the last K block's tail)
+// Forward: x = a_t, (L0, L1, c1) = (Fp, A Fp, Fp): the virtual axis is exactly the reference weight's column axis
+// [self | s-major blocks], so W_t is read as it is.  Data gradient: x = dY_t, (L0, L1, c1) = (O_t, O_t, 0): the unscaled
+// copy feeds the self columns (W_t[o, c]), the scaled ones the aggregate columns (W_t[o, Fp + s A Fp + c - Fp]); the
+// loaders put zeros in the pairs that do not meet.  The weight tiles are split hi / lo by the same threads straight from
+// W_t (no image, no workspace: the weight of one tower is a few KB and stays in L1 / L2).  Element loads are 4-byte
+// (tower widths such as 14 or 80 columns give rows that are not 16-byte aligned); 8 threads still cover 128 bytes of a row.
+// Every kLinFoldSteps K blocks the chains are folded into an fp32 register total (t = v, then t = fl(t + v) with
+// v = fl(fl(acc + corr) + b), b the bias after the last block and +0 before), in the forward as in the data gradient.
+constexpr int kTwrM = 128;                 // rows per CTA: two warpgroups of 64
+constexpr int kTwrN = 64;                  // output columns per CTA (wgmma n64)
+constexpr int kTwrSt = 2;                  // stages: {A hi, A lo, W hi, W lo}
+struct TwrSmem {
+  static constexpr int kATile = kTwrM * 128, kWTile = kTwrN * 128;
+  static constexpr int kStage = 2 * kATile + 2 * kWTile;
+  static constexpr size_t kBytes = 1024 /*align slack*/ + (size_t)kTwrSt * kStage;
+};
+
+template <bool BWD>
+__global__ void __launch_bounds__(kLinThreads, 1)
+k_towers_3xtf32(const float* __restrict__ X, long long ldx, const float* __restrict__ row_scale, int S,
+                const float* __restrict__ W, const float* __restrict__ bias, float* __restrict__ Y, long long ldy, long long N,
+                int T, int Fp, int AF, int Ot, int n_slabs) {
+  extern __shared__ unsigned char lin_raw[];
+  const unsigned base = (lin_smem_u32(lin_raw) + 1023u) & ~1023u;
+  unsigned char* gbase = lin_raw + (base - lin_smem_u32(lin_raw));
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+  // CTA -> (row tile, tower, column slab): the towers and slabs of one row tile run side by side and share its rows in L2
+  const int slab = (int)(blockIdx.x % (unsigned)n_slabs);
+  const int t = (int)(blockIdx.x / (unsigned)n_slabs % (unsigned)T);
+  const long long row0 = (long long)(blockIdx.x / (unsigned)n_slabs / (unsigned)T) * kTwrM;
+  const int L0 = BWD ? Ot : Fp, L1 = BWD ? Ot : AF, c1 = BWD ? 0 : Fp;
+  const int Kv = L0 + S * L1;                                   // virtual K
+  const int Kw = Fp + S * AF;                                   // columns of W_t
+  const int n_kb = (Kv + kLinBK - 1) / kLinBK;
+  const int n_out = BWD ? Fp + AF : Ot;                         // output columns of one tower
+  X += (long long)t * (BWD ? Ot : Fp + AF);
+  W += (long long)t * Ot * Kw;
+  Y += (long long)t * n_out + slab * kTwrN;
+  const int c_end = min(kTwrN, n_out - slab * kTwrN);           // columns of this slab that exist
+  if (bias) bias += (long long)t * Ot;
+
+  // ---- loaders: A unit (row r_in + 32 sl, 4 columns from 4 j), W units u = tid, tid + 256 (row u / 8, 4 columns from 4 (u % 8))
+  const int j = tid & 7, r_in = tid >> 3;
+  constexpr int kSlabs = kTwrM / 32;
+  float xa[kSlabs][4], xs[kSlabs][4], xw[2][4];
+  auto fetch = [&](int kb) {
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int k = kb * kLinBK + 4 * j + e;
+      int col = k, s = -1;                                      // s: scaler of the element, -1 unscaled
+      if (k >= L0) {
+        const int q = k - L0;
+        s = q / L1;
+        col = c1 + (q - s * L1);
+      }
+      const bool live = k < Kv;
+#pragma unroll
+      for (int sl = 0; sl < kSlabs; ++sl) {
+        const long long r = row0 + sl * 32 + r_in;
+        const bool ok = live && r < N;
+        xa[sl][e] = ok ? __ldg(X + r * ldx + col) : 0.f;
+        xs[sl][e] = (ok && s >= 0) ? __ldg(row_scale + r * S + s) : 1.f;
+      }
+    }
+#pragma unroll
+    for (int m = 0; m < 2; ++m) {
+      const int u = tid + m * kLinThreads, wr = u >> 3, wj = u & 7;
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int k = kb * kLinBK + 4 * wj + e;
+        float v = 0.f;
+        if (!BWD) {                                             // row wr = output o, column k of W_t
+          if (wr < Ot && k < Kv) v = __ldg(W + (long long)wr * Kw + k);
+        } else {                                                // row wr = grad_a column c of the slab, k virtual
+          const int c = slab * kTwrN + wr;
+          if (c < n_out && k < Kv) {
+            if (k < Ot) {
+              if (c < Fp) v = __ldg(W + (long long)k * Kw + c);
+            } else if (c >= Fp) {
+              const int q = k - Ot, s = q / Ot, o = q - s * Ot;
+              v = __ldg(W + (long long)o * Kw + Fp + s * AF + (c - Fp));
+            }
+          }
+        }
+        xw[m][e] = v;
+      }
+    }
+  };
+  auto store = [&](unsigned char* st) {
+#pragma unroll
+    for (int sl = 0; sl < kSlabs; ++sl) {
+      float4 hi, lo;                                            // scalers.py: src * scale, rounded to fp32 like the reference
+      lin_split(__fmul_rn(xa[sl][0], xs[sl][0]), hi.x, lo.x);   // (x * 1 == x exactly: the unscaled and the zero elements)
+      lin_split(__fmul_rn(xa[sl][1], xs[sl][1]), hi.y, lo.y);
+      lin_split(__fmul_rn(xa[sl][2], xs[sl][2]), hi.z, lo.z);
+      lin_split(__fmul_rn(xa[sl][3], xs[sl][3]), hi.w, lo.w);
+      const unsigned off = lin_swz(sl * 32 + r_in, j);
+      *reinterpret_cast<float4*>(st + off) = hi;
+      *reinterpret_cast<float4*>(st + TwrSmem::kATile + off) = lo;
+    }
+#pragma unroll
+    for (int m = 0; m < 2; ++m) {
+      const int u = tid + m * kLinThreads;
+      float4 hi, lo;
+      lin_split(xw[m][0], hi.x, lo.x);
+      lin_split(xw[m][1], hi.y, lo.y);
+      lin_split(xw[m][2], hi.z, lo.z);
+      lin_split(xw[m][3], hi.w, lo.w);
+      const unsigned off = lin_swz(u >> 3, u & 7);
+      *reinterpret_cast<float4*>(st + 2 * TwrSmem::kATile + off) = hi;
+      *reinterpret_cast<float4*>(st + 2 * TwrSmem::kATile + TwrSmem::kWTile + off) = lo;
+    }
+  };
+
+  float acc[kTwrN / 2], corr[kTwrN / 2], tot[kTwrN / 2];
+#pragma unroll
+  for (int i = 0; i < kTwrN / 2; ++i) { acc[i] = 0.f; corr[i] = 0.f; tot[i] = 0.f; }
+  const unsigned a_off = (unsigned)(wg * 64 * 128);              // warpgroup g: rows 64 g.. of the tile, all 64 columns
+  bool first = true;
+  fetch(0);
+  for (int kb = 0; kb < n_kb; ++kb) {
+    const int s = kb & 1;
+    // stage s was last read by the MMAs of step kb - 2: every warp has waited for them (wait_group 1 after step kb - 1)
+    __syncthreads();
+    store(gbase + s * TwrSmem::kStage);
+    if (kb + 1 < n_kb) fetch(kb + 1);                             // in flight while this step's MMAs run
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+    const unsigned sa = base + s * TwrSmem::kStage;
+    const unsigned a_hi = sa + a_off, a_lo = sa + TwrSmem::kATile + a_off;
+    const unsigned w_hi = sa + 2 * TwrSmem::kATile, w_lo = w_hi + TwrSmem::kWTile;
+    lin_fence_acc(acc); lin_fence_acc(corr);
+    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll
+    for (int ks = 0; ks < kLinBK / 8; ++ks) {
+      const unsigned ko = ks * 32;
+      lin_wgmma<kTwrN>(corr, lin_desc(a_hi + ko), lin_desc(w_lo + ko));
+      lin_wgmma<kTwrN>(corr, lin_desc(a_lo + ko), lin_desc(w_hi + ko));
+      lin_wgmma<kTwrN>(acc, lin_desc(a_hi + ko), lin_desc(w_hi + ko));
+    }
+    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+    if ((kb + 1) % kLinFoldSteps == 0 || kb + 1 == n_kb) {        // end of a chain: fold it into the total
+      asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+      lin_fence_acc(acc); lin_fence_acc(corr);
+      const bool last = kb + 1 == n_kb;
+#pragma unroll
+      for (int i = 0; i < kTwrN / 2; ++i) {
+        const int c = (i >> 2) * 8 + 2 * (lane & 3) + (i & 1);
+        const float b = (last && bias && c < Ot) ? __ldg(bias + c) : 0.f;
+        const float v = (acc[i] + corr[i]) + b;
+        tot[i] = first ? v : tot[i] + v;
+        acc[i] = 0.f; corr[i] = 0.f;
+      }
+      first = false;
+    } else {
+      asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+      lin_fence_acc(acc); lin_fence_acc(corr);
+    }
+  }
+  // register 4 jj + 2 h + q: row (warp % 4) * 16 + lane / 4 + 8 h of the warpgroup's 64, column 8 jj + 2 (lane % 4) + q
+  const long long r_lo = row0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+  for (int i = 0; i < kTwrN / 2; ++i) {
+    const int c = (i >> 2) * 8 + 2 * (lane & 3) + (i & 1);
+    const long long r = r_lo + 8 * ((i >> 1) & 1);
+    if (c < c_end && r < N) Y[r * ldy + c] = tot[i];
+  }
+}
+
+template <bool BWD>
+static int launch_towers(const float* X, long long ldx, const float* row_scale, int S, const float* W, const float* bias, float* Y,
+                         long long ldy, long long N, int T, int Fp, int AF, int Ot, cudaStream_t st) {
+  auto kern = k_towers_3xtf32<BWD>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    PNA_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TwrSmem::kBytes));
+    attr_set = true;
+  }
+  const int n_slabs = BWD ? (Fp + AF + kTwrN - 1) / kTwrN : 1;
+  const long long grid = (N + kTwrM - 1) / kTwrM * T * n_slabs;
+  kern<<<(unsigned)grid, kLinThreads, TwrSmem::kBytes, st>>>(X, ldx, row_scale, S, W, bias, Y, ldy, N, T, Fp, AF, Ot, n_slabs);
+  PNA_CUDA_TRY(cudaGetLastError());
+  return PNA_OK;
+}
+
 }  // namespace pna
 
 using namespace pna;
@@ -759,6 +955,45 @@ extern "C" int pna_linear_bwd_weight(const float* grad_y, int64_t ld_grad_y, con
   k_sum_splits<<<(unsigned)((n4 + 255) / 256), 256, 0, st>>>(partial, p.n_split, n4, grad_weight);
   PNA_CUDA_TRY(cudaGetLastError());
   return PNA_OK;
+}
+
+// ---- tower layers ----
+static int towers_check(int64_t n_rows, int32_t n_towers, int32_t n_feat, int32_t n_aggr, int32_t n_out, int32_t n_scalers,
+                        const char* who) {
+  PNA_REQUIRE(n_rows >= 0 && n_towers >= 1 && n_feat > 0 && n_aggr >= 1 && n_aggr <= PNA_MAX_AGGR && n_out >= 1 && n_scalers >= 1 &&
+                  n_scalers <= PNA_MAX_SCALERS,
+              PNA_ERR_BAD_ARG, "%s: bad sizes", who);
+  PNA_REQUIRE(n_towers <= 8 && n_out <= 64 && n_towers * n_out <= 256 && n_feat % 4 == 0, PNA_ERR_UNSUPPORTED,
+              "%s: needs n_towers <= 8, n_out <= 64, n_towers * n_out <= 256 and n_feat %% 4 == 0", who);
+  return PNA_OK;
+}
+
+extern "C" int pna_linear_towers_scaled_fwd(const float* a, int64_t lda, const float* row_scale, int32_t n_scalers, const float* weight,
+                                            const float* bias, float* y, int64_t ldy, int64_t n_rows, int32_t n_towers, int32_t n_feat,
+                                            int32_t n_aggr, int32_t n_out, pna_stream_t stream) {
+  const char* who = "pna_linear_towers_scaled_fwd";
+  const int rc = towers_check(n_rows, n_towers, n_feat, n_aggr, n_out, n_scalers, who);
+  if (rc != PNA_OK) return rc;
+  if (n_rows == 0) return PNA_OK;
+  PNA_REQUIRE(a && row_scale && weight && y, PNA_ERR_BAD_ARG, "%s: null pointer", who);
+  PNA_REQUIRE(lda >= (int64_t)n_towers * (1 + n_aggr) * n_feat && ldy >= (int64_t)n_towers * n_out, PNA_ERR_BAD_ARG,
+              "%s: row pitch smaller than the row", who);
+  return launch_towers<false>(a, lda, row_scale, n_scalers, weight, bias, y, ldy, n_rows, n_towers, n_feat, n_aggr * n_feat, n_out,
+                              static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int pna_linear_towers_bwd_data(const float* grad_y, int64_t ld_grad_y, const float* row_scale, int32_t n_scalers,
+                                          const float* weight, float* grad_a, int64_t ld_grad_a, int64_t n_rows, int32_t n_towers,
+                                          int32_t n_feat, int32_t n_aggr, int32_t n_out, pna_stream_t stream) {
+  const char* who = "pna_linear_towers_bwd_data";
+  const int rc = towers_check(n_rows, n_towers, n_feat, n_aggr, n_out, n_scalers, who);
+  if (rc != PNA_OK) return rc;
+  if (n_rows == 0) return PNA_OK;
+  PNA_REQUIRE(grad_y && row_scale && weight && grad_a, PNA_ERR_BAD_ARG, "%s: null pointer", who);
+  PNA_REQUIRE(ld_grad_y >= (int64_t)n_towers * n_out && ld_grad_a >= (int64_t)n_towers * (1 + n_aggr) * n_feat, PNA_ERR_BAD_ARG,
+              "%s: row pitch smaller than the row", who);
+  return launch_towers<true>(grad_y, ld_grad_y, row_scale, n_scalers, weight, nullptr, grad_a, ld_grad_a, n_rows, n_towers, n_feat,
+                             n_aggr * n_feat, n_out, static_cast<cudaStream_t>(stream));
 }
 
 namespace pna {

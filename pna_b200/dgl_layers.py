@@ -25,7 +25,7 @@ from . import _lib, padding as pad
 from .aggregate import pna_aggregate, row_scales
 from . import edge_mlp
 from .edge_mlp import edge_messages
-from .linear import compact_path_ok
+from .linear import compact_path_ok, post_linear_towers_scaled, towers_compact_pays, towers_path_ok
 from .csr import tensor_version
 from .graph import graph_csr
 from .nn_blocks import FCLayer, MLP
@@ -68,6 +68,17 @@ class PNATower(nn.Module):
             h = self.posttrans(h_cat, first_weight=w0)
         else:
             h = self.posttrans(h_cat)
+        return self._norms(h, snorm_n)
+
+    def finish_linear(self, h, snorm_n):
+        """``finish`` from the output of the first posttrans Linear (computed for every tower at once by PNALayer)."""
+        fcs = self.posttrans.fully_connected
+        h = fcs[0].after_linear(h)
+        for fc in list(fcs)[1:]:
+            h = fc(h)
+        return self._norms(h, snorm_n)
+
+    def _norms(self, h, snorm_n):
         if self.graph_norm:
             h = h * snorm_n
         if self.batch_norm:
@@ -190,6 +201,17 @@ class PNALayer(nn.Module):
             msgs.append(tw.pretrans(torch.cat(parts, dim=1)))
         return torch.cat(msgs, dim=1)
 
+    def _compact(self, h, fp: int) -> bool:
+        """Compact post path: aggregate with the identity scaler only ([N, T * (1 + A) * fp]) and let
+        pna_linear_towers_scaled_fwd form the scaled copies in registers -- the [N, T * (1 + S*A) * fp] tensor is never
+        written, nor saved for the backward.  Same arithmetic; float32 with more than one scaler, at the kernel's shapes,
+        in training steps on graphs of at least linear.TOWERS_COMPACT_MIN_ROWS rows, where it measured faster."""
+        fc0 = self.towers[0].posttrans.fully_connected[0].linear
+        training = torch.is_grad_enabled() and any(p_.requires_grad for p_ in self.parameters())
+        return fc0.weight.dtype == torch.float32 and fc0.bias is not None and \
+            towers_path_ok(h, len(self.towers), fp, self.output_tower, len(self.scalers)) and \
+            towers_compact_pays(h.size(0), training)
+
     def forward(self, g, h, e, snorm_n):
         h_in = h
         csr = graph_csr(g, h.device)
@@ -202,18 +224,29 @@ class PNALayer(nn.Module):
         else:
             h_self = pad.pad_cols(h, fp)
         common = dict(towers=T, self_feat=h_self, self_divided=self.divide_input, zero_isolated=True, relu_var=True)
+        compact = self._compact(h, fp)
+        scalers = ["identity"] if compact else self.scalers
         if not self.edge_features and self.towers[0].pretrans.is_single_affine():
             U, V = self._affine_terms(h, fp)
-            agg = pna_aggregate(V, csr, self.aggregators, self.scalers, self.avg_d, row_bias=U, **common)
+            agg = pna_aggregate(V, csr, self.aggregators, scalers, self.avg_d, row_bias=U, **common)
         else:
             if self._fused_messages_ok(h, e, csr.n_edges):
                 msgs = self._fused_messages(csr, h, e, fp)
             else:
                 msgs = pad.pad_blocks(self._edge_messages(csr, h, e), T, it, fp)
-            agg = pna_aggregate(msgs, csr, self.aggregators, self.scalers, self.avg_d, messages_in_csr_order=True, **common)
-        agg = agg.view(h.size(0), T, -1)                                  # [N, T, (1 + S*A) * fp] = cat([h_t, reduced])
+            agg = pna_aggregate(msgs, csr, self.aggregators, scalers, self.avg_d, messages_in_csr_order=True, **common)
         blocks = 1 + len(self.aggregators) * len(self.scalers)
-        h_cat = torch.cat([tw.finish(agg[:, t], snorm_n, blocks, fp) for t, tw in enumerate(self.towers)], dim=1)
+        if compact:
+            # compact post path: [N, T, (1 + A) * fp] aggregate, every tower's first posttrans Linear in one kernel that
+            # forms the scaled copies in registers; the rest of each tower's posttrans and norms on its output_tower slice
+            lins = [tw.posttrans.fully_connected[0].linear for tw in self.towers]
+            w0 = torch.stack([pad.expand_weight_cols(l.weight, blocks, it, fp) for l in lins])
+            y = post_linear_towers_scaled(agg, row_scales(csr, self.scalers, self.avg_d), w0, torch.stack([l.bias for l in lins]))
+            ot = self.output_tower
+            h_cat = torch.cat([tw.finish_linear(y[:, t * ot:(t + 1) * ot], snorm_n) for t, tw in enumerate(self.towers)], dim=1)
+        else:
+            agg = agg.view(h.size(0), T, -1)                              # [N, T, (1 + S*A) * fp] = cat([h_t, reduced])
+            h_cat = torch.cat([tw.finish(agg[:, t], snorm_n, blocks, fp) for t, tw in enumerate(self.towers)], dim=1)
         h_out = self.mixing_network(h_cat)
         if self.residual:
             h_out = h_in + h_out

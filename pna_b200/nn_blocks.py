@@ -57,6 +57,10 @@ class FCLayer(nn.Module):
             h = post_linear(x, self.linear.weight if weight is None else weight, self.linear.bias)
         else:
             h = self.linear(x) if weight is None else nn.functional.linear(x, weight, self.linear.bias)
+        return self.after_linear(h)
+
+    def after_linear(self, h):
+        """activation -> dropout -> batch norm on the output of this layer's Linear (computed by the caller)."""
         if self.activation is not None:
             h = self.activation(h)
         if self.dropout is not None:

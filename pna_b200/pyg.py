@@ -17,7 +17,7 @@ from . import _lib, padding as pad
 from .aggregate import avg_deg_from_histogram, pna_aggregate, row_scales
 from . import edge_mlp
 from .edge_mlp import edge_messages
-from .linear import compact_path_ok, linear_tf32x3, post_linear, post_linear_scaled
+from .linear import compact_path_ok, linear_tf32x3, post_linear, post_linear_scaled, post_linear_towers_scaled, towers_compact_pays, towers_path_ok
 from .csr import CSRGraph, csr_from_edge_index, tensor_version
 
 _AGGRS = ("sum", "mean", "min", "max", "var", "std")          # aggregators.py:35-42
@@ -379,6 +379,16 @@ class PNAConv(Module):
         h = linear_tf32x3(buf, tc["w2"], tc["b2"])                                               # [N, O2] = cat over towers | 0
         return linear_tf32x3(h, tc["w3"], tc["b3"])[:, : self.out_channels]
 
+    def _compact(self, x: Tensor, Fp: int) -> bool:
+        """Compact post path (taken wherever _forward_tensor_cores is not): aggregate with the identity scaler only
+        ([N, T*(1 + A)*Fp]) and let pna_linear_towers_scaled_fwd form the scaled copies in registers -- the
+        [N, T*(1 + S*A)*Fp] tensor is never written, nor saved for the backward.  Same arithmetic.  Training steps on
+        graphs of at least linear.TOWERS_COMPACT_MIN_ROWS rows, where it measured faster."""
+        w = self.post_nns[0][0].weight
+        training = torch.is_grad_enabled() and any(p_.requires_grad for p_ in self.parameters())
+        return (w.dtype == torch.float32 and towers_path_ok(x, self.towers, Fp, self.F_out, len(self.scalers))
+                and towers_compact_pays(x.size(0), training))
+
     def forward(self, x: Tensor, edge_index: Tensor, edge_attr: Optional[Tensor] = None, *,
                 deg: Optional[Tensor] = None, csr: Optional[CSRGraph] = None) -> Tensor:
         csr = _resolve_csr(x, edge_index, csr)
@@ -394,18 +404,28 @@ class PNAConv(Module):
         if self._tensor_core_ok(x, edge_attr, Fp):
             return self._forward_tensor_cores(x, csr, x_self, Fp)
         common = dict(towers=T, self_feat=x_self, self_divided=self.divide_input)
+        compact = self._compact(x, Fp)
+        scalers = ["identity"] if compact else self.scalers
         if edge_attr is None and self.pre_layers == 1 and self.edge_dim is None:
             U, V = self._affine_terms(x, Fp)
-            out = pna_aggregate(V, csr, self.aggregators, self.scalers, self.avg_deg, row_bias=U, **common)
+            out = pna_aggregate(V, csr, self.aggregators, scalers, self.avg_deg, row_bias=U, **common)
         else:
             if self._fused_messages_ok(x, edge_attr, csr.n_edges):
                 msgs = self._fused_messages(x, csr, edge_attr, Fp)
             else:
                 msgs = pad.pad_blocks(self._messages_in_slot_order(x, csr, edge_attr), T, Fi, Fp)
-            out = pna_aggregate(msgs, csr, self.aggregators, self.scalers, self.avg_deg, messages_in_csr_order=True,
+            out = pna_aggregate(msgs, csr, self.aggregators, scalers, self.avg_deg, messages_in_csr_order=True,
                                 **common)
-        out = out.view(x.size(0), T, -1)                       # [N, T, (1 + S*A) * Fp]  (pna.py:131)
         w_post, b_post = self._prepared(Fp)[2:]
+        if compact:
+            # [N, T*(1 + A)*Fp] -> first post Linear of every tower in one kernel (the scaled copies in its registers),
+            # already the concatenation over the towers (pna.py:134)
+            h = post_linear_towers_scaled(out, row_scales(csr, self.scalers, self.avg_deg), w_post, b_post)
+            if len(self.post_nns[0]) > 1:
+                Fo = self.F_out
+                h = torch.cat([self._rest(nn, h[:, t * Fo:(t + 1) * Fo]) for t, nn in enumerate(self.post_nns)], dim=1)
+            return self.lin(h)
+        out = out.view(x.size(0), T, -1)                       # [N, T, (1 + S*A) * Fp]  (pna.py:131)
         # first post Linear of all towers: one batched GEMM on the [N, T, W] view (tower = batch, no copy of the big tensor)
         h = torch.baddbmm(b_post.unsqueeze(1), out.transpose(0, 1), w_post.transpose(1, 2))      # [T, N, F_out]
         if len(self.post_nns[0]) > 1:
