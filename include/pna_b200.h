@@ -291,7 +291,8 @@ int pna_aggregate_bwd_combine(const float* coef_sums, int64_t ld_sums, int32_t c
  *     path adds into grad_gathered[col[slot]], bit for bit -- and writes columns [f_begin, f_begin + f_count) of
  *     grad_row_bias (nullable, [n_rows, n_feat] fp32, addressed like pna_aggregate_bwd's), split rows as the chunks' slot-order
  *     sums added in chunk order.  With desc->col == NULL (messages in CSR order) grad_slots IS the gradient of the messages.
- *     desc->hub_partials as for pna_aggregate_bwd.  Peer-memory descriptors: PNA_ERR_UNSUPPORTED.
+ *     desc->hub_partials as for pna_aggregate_bwd.  Peer-memory descriptors: PNA_ERR_UNSUPPORTED (they take
+ *     pna_aggregate_bwd_peer_slots below).
  *  2. (desc->col != NULL) the caller sums grad_slots over the out-edges of every source row: pna_aggregate_fwd on the
  *     slot-transposed CSR (pna_csr_build with src = slot id 0..E-1, dst = col, n_nodes = n_src: rows are source rows, slots
  *     are forward slot ids in ascending order) with gathered = grad_slots, one aggregator PNA_AGGR_SUM, one scaler
@@ -299,6 +300,18 @@ int pna_aggregate_bwd_combine(const float* coef_sums, int64_t ld_sums, int32_t c
 int pna_aggregate_bwd_slots(const pna_agg_t* desc, const void* grad_out, int64_t ld_grad_out, int32_t f_begin, int32_t f_count,
                             float* grad_slots, int64_t ld_grad_slots, float* grad_row_bias, int64_t ld_grad_row_bias,
                             pna_stream_t stream);
+
+/* Step 1 of pna_aggregate_bwd_slots for a peer-memory graph (desc->peer_gathered != NULL, required: PNA_ERR_BAD_ARG
+ * otherwise): the source row of slot s is row (col[s] & mask) of rank (col[s] >> peer_shift), read over NVLink as
+ * pna_aggregate_fwd reads it.  Same arguments, slab rules and results: grad_slots row s and grad_row_bias are the bits
+ * pna_aggregate_bwd_slots stores for the same slot of the unpartitioned graph; no floating-point atomics.  What the peer
+ * forward refuses is refused here: moment, softmax / softmin / normalised_mean aggregators and row_ids
+ * (PNA_ERR_UNSUPPORTED), and col == NULL (PNA_ERR_UNSUPPORTED).  Every rank's gathered rows must stay unchanged until all
+ * ranks' calls that read them have completed.  Step 2 is the owners': each adds the slots that name its rows into its
+ * own gradient (pna_halo_grad_pull over the ranks' grad_slots buffers, slots in ascending (rank, slot) order). */
+int pna_aggregate_bwd_peer_slots(const pna_agg_t* desc, const void* grad_out, int64_t ld_grad_out, int32_t f_begin,
+                                 int32_t f_count, float* grad_slots, int64_t ld_grad_slots, float* grad_row_bias,
+                                 int64_t ld_grad_row_bias, pna_stream_t stream);
 
 /* ---- the per-edge pretrans MLP of the dense layer with pretrans_layers = L >= 2 (models/layers.py:200-229) ------------
  * For every slot s of a destination-sorted CSR (row i, source j = col[s]) and tower t (all fp32, row-major, contiguous,

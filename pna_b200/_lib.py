@@ -47,7 +47,7 @@ EDGE_MLP_MAX_WIDTH = 64      # PNA_EDGE_MLP_MAX_WIDTH
 
 # every symbol the header declares (checked by tests/test_abi.py)
 EXPORTED_SYMBOLS = ("pna_csr_workspace_bytes", "pna_csr_build", "pna_csr_light_view", "pna_csr_light_view_workspace_bytes", "pna_aggregate_fwd", "pna_aggregate_bwd",
-                    "pna_aggregate_bwd_coef", "pna_aggregate_bwd_combine", "pna_aggregate_bwd_slots",
+                    "pna_aggregate_bwd_coef", "pna_aggregate_bwd_combine", "pna_aggregate_bwd_slots", "pna_aggregate_bwd_peer_slots",
                     "pna_gather_rows", "pna_halo_pull", "pna_halo_grad_pull", "pna_peer_barrier", "pna_linear_fwd", "pna_linear_scaled_fwd", "pna_row_scales", "pna_linear_workspace_bytes",
                     "pna_linear_bwd_workspace_bytes", "pna_linear_bwd_data", "pna_linear_bwd_weight", "pna_edge_mlp_fwd",
                     "pna_edge_mlp_bwd", "pna_edge_msg_fwd", "pna_edge_msg_bwd", "pna_query", "pna_last_error",
@@ -181,6 +181,8 @@ def lib() -> C.CDLL:
         L.pna_aggregate_bwd_slots.restype = C.c_int
         L.pna_aggregate_bwd_slots.argtypes = [C.POINTER(AggStruct), C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_int64,
                                               C.c_void_p, C.c_int64, C.c_void_p]
+        L.pna_aggregate_bwd_peer_slots.restype = C.c_int
+        L.pna_aggregate_bwd_peer_slots.argtypes = L.pna_aggregate_bwd_slots.argtypes
         L.pna_gather_rows.restype = C.c_int
         L.pna_gather_rows.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32,
                                       C.c_int32, C.c_void_p]

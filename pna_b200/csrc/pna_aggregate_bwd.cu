@@ -24,6 +24,14 @@
 // grad_gathered[col[slot]]; the caller sums those rows over the reversed edges with the forward kernel (fixed order).  Split
 // rows store each chunk's share of grad_row_bias in scratch and k_bwd_hub_bias adds the shares in chunk order.  No
 // floating-point atomics in any kernel of this variant.
+//
+// pna_aggregate_bwd_peer_slots (the peer plane's backward): the bodies of the per-slot kernels that read source rows
+// (bwd_rows, bwd_hub_stats, bwd_hub_scatter) compiled with PEER = true into k_peer_bwd_*, so that col = owner << shift |
+// row is read from the owner's buffer through the peer pointer table (NVLink) exactly as the forward's PEER instances
+// read it.  Nothing else differs: each slot's gradient and grad_row_bias are the
+// bits pna_aggregate_bwd_slots stores for the same slot of the unpartitioned graph.  k_bwd_hub_coef and k_bwd_hub_bias
+// read only scratch and grad_out, so their per-slot instances serve both.  The existing k_bwd_* kernels are thin wrappers
+// around the same bodies with PEER = false: their symbols and SASS are what they were before the peer instances existed.
 #include "pna_aggregate.cuh"
 #include <string.h>
 
@@ -71,6 +79,14 @@ template <int VEC>
 struct Coef {
   float c0[VEC], c1[VEC], gmin[VEC], gmax[VEC];
 };
+
+// Source row `c` of a slot.  PEER (pna_aggregate_bwd_peer_slots): c = owner << shift | row, read from the owner's buffer
+// through the peer pointer table as the forward's PEER instances read it; otherwise a row of the local buffer.
+template <typename T, bool PEER>
+__device__ __forceinline__ const T* source_row(const KParams& p, int c) {
+  if constexpr (PEER) return gathered_row<T>(p, c);
+  else return local_row<T>(p, c);
+}
 
 template <typename T, int VEC>
 __device__ __forceinline__ void load_m(const KParams& p, int src, int f, const float (&bias)[VEC], bool has_bias, float (&m)[VEC]) {
@@ -234,8 +250,8 @@ __device__ __forceinline__ void emit_row(const BParams& b, long long row, int de
 constexpr int kBwdThreads = 256;
 
 // ---- rows below the split threshold: one lane group per row --------------------------------------------------------
-template <typename T, int VEC, int G, bool SLOTS>
-__global__ void __launch_bounds__(kBwdThreads) k_bwd_rows(const BParams b) {
+template <typename T, int VEC, int G, bool SLOTS, bool PEER>
+__device__ __forceinline__ void bwd_rows(const BParams& b) {
   const KParams& p = b.k;
   constexpr int RPW = 32 / G;
   const int lane = threadIdx.x & 31, gl = lane % G;
@@ -267,7 +283,7 @@ __global__ void __launch_bounds__(kBwdThreads) k_bwd_rows(const BParams b) {
 #pragma unroll
     for (int u = 0; u < UB; ++u) src[u] = (e + u < end) ? (p.col ? __ldg(p.col + e + u) : e + u) : -1;
 #pragma unroll
-    for (int u = 0; u < UB; ++u) if (src[u] >= 0) raw[u] = Io<T, VEC>::load_raw(local_row<T>(p, src[u]) + lc.f);
+    for (int u = 0; u < UB; ++u) if (src[u] >= 0) raw[u] = Io<T, VEC>::load_raw(source_row<T, PEER>(p, src[u]) + lc.f);
 #pragma unroll
     for (int u = 0; u < UB; ++u) {
       if (src[u] >= 0) {
@@ -298,7 +314,7 @@ __global__ void __launch_bounds__(kBwdThreads) k_bwd_rows(const BParams b) {
 #pragma unroll
     for (int u = 0; u < UB; ++u) src[u] = (e + u < end) ? (p.col ? __ldg(p.col + e + u) : e + u) : -1;
 #pragma unroll
-    for (int u = 0; u < UB; ++u) if (src[u] >= 0) raw[u] = Io<T, VEC>::load_raw(local_row<T>(p, src[u]) + lc.f);
+    for (int u = 0; u < UB; ++u) if (src[u] >= 0) raw[u] = Io<T, VEC>::load_raw(source_row<T, PEER>(p, src[u]) + lc.f);
 #pragma unroll
     for (int u = 0; u < UB; ++u) {
       if (src[u] >= 0) {
@@ -321,6 +337,13 @@ __global__ void __launch_bounds__(kBwdThreads) k_bwd_rows(const BParams b) {
   }
 }
 
+template <typename T, int VEC, int G, bool SLOTS>
+__global__ void __launch_bounds__(kBwdThreads) k_bwd_rows(const BParams b) { bwd_rows<T, VEC, G, SLOTS, false>(b); }
+
+// the peer plane's instance (pna_aggregate_bwd_peer_slots): per-slot, source rows read through the peer pointer table
+template <typename T, int VEC, int G>
+__global__ void __launch_bounds__(kBwdThreads) k_peer_bwd_rows(const BParams b) { bwd_rows<T, VEC, G, true, true>(b); }
+
 // ---- split rows: chunk-parallel, like the forward ---------------------------------------------------------------
 // (1) k_bwd_hub_stats: one lane group per 128-slot chunk -> partial sum, sumsq, min, max, first argmin / argmax slot;
 // (2) k_bwd_hub_coef:  one lane group per split row merges its chunks in chunk order (strict < keeps the first slot)
@@ -329,8 +352,8 @@ __global__ void __launch_bounds__(kBwdThreads) k_bwd_rows(const BParams b) {
 //                      row_bias gradient.  Scratch (descriptor field hub_partials): 6*F floats per chunk + per split row.
 // Per-slot mode: (3) stores grad_m per slot and parks the chunk's row_bias share in the chunk's (consumed) sum partial;
 // (4) k_bwd_hub_bias: one lane group per split row adds those shares in chunk order.
-template <typename T, int VEC, int G, bool SLOTS>
-__global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_stats(const BParams b) {
+template <typename T, int VEC, int G, bool SLOTS, bool PEER>
+__device__ __forceinline__ void bwd_hub_stats(const BParams& b) {
   const KParams& p = b.k;
   constexpr int RPW = 32 / G;
   const int lane = threadIdx.x & 31, gl = lane % G;
@@ -354,7 +377,7 @@ __global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_stats(const BParams b) 
 #pragma unroll
     for (int u = 0; u < UB; ++u) src[u] = (e + u < end) ? (p.col ? __ldg(p.col + e + u) : e + u) : -1;
 #pragma unroll
-    for (int u = 0; u < UB; ++u) if (src[u] >= 0) raw[u] = Io<T, VEC>::load_raw(local_row<T>(p, src[u]) + lc.f);
+    for (int u = 0; u < UB; ++u) if (src[u] >= 0) raw[u] = Io<T, VEC>::load_raw(source_row<T, PEER>(p, src[u]) + lc.f);
 #pragma unroll
     for (int u = 0; u < UB; ++u) {
       if (src[u] >= 0) {
@@ -375,6 +398,13 @@ __global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_stats(const BParams b) 
     part[4ll * p.F + i] = __int_as_float(st.amn[i]); part[5ll * p.F + i] = __int_as_float(st.amx[i]);
   }
 }
+
+template <typename T, int VEC, int G, bool SLOTS>
+__global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_stats(const BParams b) { bwd_hub_stats<T, VEC, G, SLOTS, false>(b); }
+
+// the peer plane's instance (pna_aggregate_bwd_peer_slots): per-slot, source rows read through the peer pointer table
+template <typename T, int VEC, int G>
+__global__ void __launch_bounds__(kBwdThreads) k_peer_bwd_hub_stats(const BParams b) { bwd_hub_stats<T, VEC, G, true, true>(b); }
 
 template <typename T, int VEC, int G, bool SLOTS>
 __global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_coef(const BParams b) {
@@ -426,8 +456,8 @@ __global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_coef(const BParams b) {
   }
 }
 
-template <typename T, int VEC, int G, bool SLOTS>
-__global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_scatter(const BParams b) {
+template <typename T, int VEC, int G, bool SLOTS, bool PEER>
+__device__ __forceinline__ void bwd_hub_scatter(const BParams& b) {
   const KParams& p = b.k;
   constexpr int RPW = 32 / G;
   const int lane = threadIdx.x & 31, gl = lane % G;
@@ -460,7 +490,7 @@ __global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_scatter(const BParams b
 #pragma unroll
     for (int u = 0; u < UB; ++u) src[u] = (e + u < end) ? (p.col ? __ldg(p.col + e + u) : e + u) : -1;
 #pragma unroll
-    for (int u = 0; u < UB; ++u) if (src[u] >= 0) raw[u] = Io<T, VEC>::load_raw(local_row<T>(p, src[u]) + lc.f);
+    for (int u = 0; u < UB; ++u) if (src[u] >= 0) raw[u] = Io<T, VEC>::load_raw(source_row<T, PEER>(p, src[u]) + lc.f);
 #pragma unroll
     for (int u = 0; u < UB; ++u) {
       if (src[u] >= 0) {
@@ -489,6 +519,13 @@ __global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_scatter(const BParams b
   }
 }
 
+template <typename T, int VEC, int G, bool SLOTS>
+__global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_scatter(const BParams b) { bwd_hub_scatter<T, VEC, G, SLOTS, false>(b); }
+
+// the peer plane's instance (pna_aggregate_bwd_peer_slots): per-slot, source rows read through the peer pointer table
+template <typename T, int VEC, int G>
+__global__ void __launch_bounds__(kBwdThreads) k_peer_bwd_hub_scatter(const BParams b) { bwd_hub_scatter<T, VEC, G, true, true>(b); }
+
 // per-slot mode, split rows: grad_row_bias = the chunks' shares added in chunk order (each share in slot order)
 template <int VEC, int G>
 __global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_bias(const BParams b) {
@@ -513,8 +550,9 @@ __global__ void __launch_bounds__(kBwdThreads) k_bwd_hub_bias(const BParams b) {
   for (int i = 0; i < VEC; ++i) b.gb[row * b.ldgb + lc.f + i] = acc[i];
 }
 
-template <typename T, int VEC, int G, bool SLOTS>
+template <typename T, int VEC, int G, bool SLOTS, bool PEER>
 static int launch_bwd(const BParams& b, cudaStream_t st) {
+  static_assert(SLOTS || !PEER, "peer-memory graphs have the per-slot backward only");
   const KParams& p = b.k;
   constexpr int RPW = 32 / G;
   const int width = SLOTS ? b.f1 - b.f0 : p.F;     // the per-slot mode covers one feature slab
@@ -522,16 +560,25 @@ static int launch_bwd(const BParams& b, cudaStream_t st) {
   const long long per_block = (kBwdThreads / 32) * RPW;
   const long long gx = (p.n_rows + per_block - 1) / per_block;
   PNA_REQUIRE(gx <= 0x7fffffffll, PNA_ERR_UNSUPPORTED, "pna_aggregate_bwd: too many rows");
-  k_bwd_rows<T, VEC, G, SLOTS><<<dim3((unsigned)gx, gy), kBwdThreads, 0, st>>>(b);
+  if constexpr (PEER)
+    k_peer_bwd_rows<T, VEC, G><<<dim3((unsigned)gx, gy), kBwdThreads, 0, st>>>(b);
+  else
+    k_bwd_rows<T, VEC, G, SLOTS><<<dim3((unsigned)gx, gy), kBwdThreads, 0, st>>>(b);
   PNA_CUDA_TRY(cudaGetLastError());
   if (p.n_hubs > 0) {
     const long long gc = (p.n_chunks + per_block - 1) / per_block, gh = (p.n_hubs + per_block - 1) / per_block;
-    k_bwd_hub_stats<T, VEC, G, SLOTS><<<dim3((unsigned)gc, gy), kBwdThreads, 0, st>>>(b);
+    if constexpr (PEER)
+      k_peer_bwd_hub_stats<T, VEC, G><<<dim3((unsigned)gc, gy), kBwdThreads, 0, st>>>(b);
+    else
+      k_bwd_hub_stats<T, VEC, G, SLOTS><<<dim3((unsigned)gc, gy), kBwdThreads, 0, st>>>(b);
     PNA_CUDA_TRY(cudaGetLastError());
     k_bwd_hub_coef<T, VEC, G, SLOTS><<<dim3((unsigned)gh, gy), kBwdThreads, 0, st>>>(b);
     PNA_CUDA_TRY(cudaGetLastError());
     if (!b.coef) {
-      k_bwd_hub_scatter<T, VEC, G, SLOTS><<<dim3((unsigned)gc, gy), kBwdThreads, 0, st>>>(b);
+      if constexpr (PEER)
+        k_peer_bwd_hub_scatter<T, VEC, G><<<dim3((unsigned)gc, gy), kBwdThreads, 0, st>>>(b);
+      else
+        k_bwd_hub_scatter<T, VEC, G, SLOTS><<<dim3((unsigned)gc, gy), kBwdThreads, 0, st>>>(b);
       PNA_CUDA_TRY(cudaGetLastError());
     }
     if (SLOTS && b.gb) {
@@ -542,15 +589,15 @@ static int launch_bwd(const BParams& b, cudaStream_t st) {
   return PNA_OK;
 }
 
-template <typename T, int VEC, bool SLOTS>
+template <typename T, int VEC, bool SLOTS, bool PEER = false>
 static int launch_bwd_typed(const BParams& b, cudaStream_t st) {
   const int chunks = (SLOTS ? b.f1 - b.f0 : b.k.F) / VEC;
-  if (chunks <= 1) return launch_bwd<T, VEC, 1, SLOTS>(b, st);
-  if (chunks <= 2) return launch_bwd<T, VEC, 2, SLOTS>(b, st);
-  if (chunks <= 4) return launch_bwd<T, VEC, 4, SLOTS>(b, st);
-  if (chunks <= 8) return launch_bwd<T, VEC, 8, SLOTS>(b, st);
-  if (chunks <= 16) return launch_bwd<T, VEC, 16, SLOTS>(b, st);
-  return launch_bwd<T, VEC, 32, SLOTS>(b, st);     // wider rows: several feature blocks (gridDim.y)
+  if (chunks <= 1) return launch_bwd<T, VEC, 1, SLOTS, PEER>(b, st);
+  if (chunks <= 2) return launch_bwd<T, VEC, 2, SLOTS, PEER>(b, st);
+  if (chunks <= 4) return launch_bwd<T, VEC, 4, SLOTS, PEER>(b, st);
+  if (chunks <= 8) return launch_bwd<T, VEC, 8, SLOTS, PEER>(b, st);
+  if (chunks <= 16) return launch_bwd<T, VEC, 16, SLOTS, PEER>(b, st);
+  return launch_bwd<T, VEC, 32, SLOTS, PEER>(b, st);     // wider rows: several feature blocks (gridDim.y)
 }
 
 static bool al16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15u) == 0; }
@@ -653,11 +700,12 @@ __global__ void __launch_bounds__(256) k_bwd_combine(const float* __restrict__ s
 
 using namespace pna;
 
-// grad_slots != NULL: the per-slot mode (pna_aggregate_bwd_slots) over the feature slab [f_begin, f_begin + f_count)
+// grad_slots != NULL: the per-slot mode (pna_aggregate_bwd_slots) over the feature slab [f_begin, f_begin + f_count);
+// peer: the same over a peer-memory graph (pna_aggregate_bwd_peer_slots), source rows read through desc->peer_gathered
 static int bwd_entry(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_out, float* grad_gathered, int64_t ld_grad_gathered,
                      float* grad_row_bias, int64_t ld_grad_row_bias, float* coef, int64_t ld_coef, int32_t coef_c1,
                      pna_stream_t stream, float* grad_slots = nullptr, int64_t ld_grad_slots = 0, int32_t f_begin = 0,
-                     int32_t f_count = 0) {
+                     int32_t f_count = 0, bool peer = false) {
   PNA_REQUIRE(d != nullptr, PNA_ERR_BAD_ARG, "pna_aggregate_bwd: null descriptor");
   PNA_REQUIRE(d->n_rows >= 0 && d->n_feat > 0 && d->n_towers > 0 && d->n_feat % d->n_towers == 0, PNA_ERR_BAD_ARG,
               "pna_aggregate_bwd: bad sizes");
@@ -690,7 +738,16 @@ static int bwd_entry(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_o
               PNA_ERR_UNSUPPORTED, "pna_aggregate_bwd: normalised_mean needs col or degree_col (the source of every slot)");
   if (d->n_rows == 0) return PNA_OK;
   PNA_REQUIRE(d->gathered && d->rowptr && grad_out && (slots || grad_gathered), PNA_ERR_BAD_ARG, "pna_aggregate_bwd: null pointer");
-  PNA_REQUIRE(d->peer_gathered == nullptr, PNA_ERR_UNSUPPORTED, "pna_aggregate_bwd: peer-memory graphs are forward-only");
+  if (peer) {
+    PNA_REQUIRE(d->peer_gathered != nullptr, PNA_ERR_BAD_ARG, "pna_aggregate_bwd_peer_slots: no peer_gathered table");
+    PNA_REQUIRE(d->peer_shift >= 1 && d->peer_shift <= 30, PNA_ERR_BAD_ARG, "pna_aggregate_bwd_peer_slots: peer_shift out of range");
+    PNA_REQUIRE(d->row_ids == nullptr, PNA_ERR_UNSUPPORTED, "pna_aggregate_bwd_peer_slots: row_ids are not available");
+    PNA_REQUIRE(d->col != nullptr, PNA_ERR_UNSUPPORTED,
+                "pna_aggregate_bwd_peer_slots: col is required (it names the owner and row of every source)");
+  } else {
+    PNA_REQUIRE(d->peer_gathered == nullptr, PNA_ERR_UNSUPPORTED,
+                "pna_aggregate_bwd: peer-memory graphs have pna_aggregate_bwd_peer_slots only");
+  }
   PNA_REQUIRE(d->ld_gathered < 0x3fffffffll, PNA_ERR_UNSUPPORTED, "pna_aggregate_bwd: row pitch too large");
   PNA_REQUIRE(d->split_threshold >= 2, PNA_ERR_BAD_ARG, "pna_aggregate_bwd: bad split threshold");
   if (d->n_hubs > 0)
@@ -714,6 +771,7 @@ static int bwd_entry(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_o
   p.hub_info = d->hub_info; p.n_hubs = d->n_hubs; p.chunk_items = d->chunk_items; p.n_chunks = d->n_chunks;
   p.partials = d->hub_partials;
   p.sdeg = d->scaler_degree;
+  if (peer) { p.peer_x = reinterpret_cast<const void* const*>(d->peer_gathered); p.peer_shift = d->peer_shift; }
   b.go = grad_out; b.ldgo = ld_grad_out;
   b.gg = grad_gathered; b.ldgg = ld_grad_gathered;
   b.gb = grad_row_bias; b.ldgb = ld_grad_row_bias;
@@ -739,7 +797,10 @@ static int bwd_entry(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_o
   if (p.bias) vec_ok = vec_ok && al16(p.bias) && (p.ldb % vec == 0);
   const bool f32 = d->dtype == PNA_F32;
   int rc;
-  if (slots) {
+  if (peer) {
+    if (f32) rc = vec_ok ? launch_bwd_typed<float, 4, true, true>(b, st) : launch_bwd_typed<float, 1, true, true>(b, st);
+    else rc = vec_ok ? launch_bwd_typed<__nv_bfloat16, 8, true, true>(b, st) : launch_bwd_typed<__nv_bfloat16, 1, true, true>(b, st);
+  } else if (slots) {
     if (f32) rc = vec_ok ? launch_bwd_typed<float, 4, true>(b, st) : launch_bwd_typed<float, 1, true>(b, st);
     else rc = vec_ok ? launch_bwd_typed<__nv_bfloat16, 8, true>(b, st) : launch_bwd_typed<__nv_bfloat16, 1, true>(b, st);
   } else {
@@ -770,6 +831,14 @@ extern "C" int pna_aggregate_bwd_slots(const pna_agg_t* d, const void* grad_out,
   PNA_REQUIRE(grad_slots != nullptr, PNA_ERR_BAD_ARG, "pna_aggregate_bwd_slots: null grad_slots");
   return bwd_entry(d, grad_out, ld_grad_out, nullptr, 0, grad_row_bias, ld_grad_row_bias, nullptr, 0, 0, stream, grad_slots,
                    ld_grad_slots, f_begin, f_count);
+}
+
+extern "C" int pna_aggregate_bwd_peer_slots(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_out, int32_t f_begin,
+                                            int32_t f_count, float* grad_slots, int64_t ld_grad_slots, float* grad_row_bias,
+                                            int64_t ld_grad_row_bias, pna_stream_t stream) {
+  PNA_REQUIRE(grad_slots != nullptr, PNA_ERR_BAD_ARG, "pna_aggregate_bwd_peer_slots: null grad_slots");
+  return bwd_entry(d, grad_out, ld_grad_out, nullptr, 0, grad_row_bias, ld_grad_row_bias, nullptr, 0, 0, stream, grad_slots,
+                   ld_grad_slots, f_begin, f_count, true);
 }
 
 extern "C" int pna_aggregate_bwd_coef(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_out, float* coef, int64_t ld_coef,

@@ -26,6 +26,7 @@ it without GPUs.
 """
 from __future__ import annotations
 
+import ctypes as C
 from dataclasses import dataclass
 from typing import List, Optional
 
@@ -33,7 +34,7 @@ import torch
 import torch.distributed as dist
 
 from . import _lib
-from .aggregate import aggregate_forward, pna_aggregate
+from .aggregate import _DTYPES, _names, _rows2d, aggregate_forward, deterministic_slab_width, pna_aggregate
 from .csr import LightView, build_csr
 
 
@@ -320,6 +321,8 @@ class GradReturnPlan:
     # pull plane only: every rank's n_local, where its halo-gradient rows start in its [local ; halo] buffer.  None in the
     # halo plane's plan (halo_grad_return_plan), whose segments are the peers' parts of the local receive buffer.
     peer_n_local: Optional[List[int]] = None
+    # peer plane only (peer_grad_return_plan): every rank's number of CSR slots, which sizes the per-slot gradient buffers
+    peer_n_edges: Optional[List[int]] = None
 
     @property
     def n_rows(self) -> int:
@@ -357,17 +360,95 @@ def grad_return_plan(rank: int, world: int, held: List[torch.Tensor], offsets: L
         rows_l.append(ids)
         enc_l.append((p << shift) | pos)
     n_local = None if peer_n_local is None else list(map(int, peer_n_local))
+    return _reverse_csr(rank, world, shift, rows_l, enc_l, device, peer_n_local=n_local)
+
+
+def _reverse_csr(rank: int, world: int, shift: int, rows_l: List[torch.Tensor], enc_l: List[torch.Tensor], device,
+                 **extra) -> GradReturnPlan:
+    """The plan's CSR from per-peer (rows, encoded slots) lists appended in ascending peer rank: rows grouped, each row's
+    slots kept in the order they were appended (stable sort)."""
     if not rows_l:
         empty = torch.zeros(0, dtype=torch.int32, device=device)
         return GradReturnPlan(rank, world, shift, empty, torch.zeros(1, dtype=torch.int32, device=device), empty.clone(),
-                              n_local)
+                              **extra)
     rows, enc = torch.cat(rows_l), torch.cat(enc_l)
     order = torch.sort(rows, stable=True).indices          # peers were appended in rank order: stable keeps it per row
     rows, enc = rows[order], enc[order]
     uniq, counts = torch.unique_consecutive(rows, return_counts=True)
     rowptr = torch.zeros(uniq.numel() + 1, dtype=torch.int64, device=device)
     rowptr[1:] = torch.cumsum(counts, 0)
-    return GradReturnPlan(rank, world, shift, uniq.to(torch.int32), rowptr.to(torch.int32), enc.to(torch.int32), n_local)
+    return GradReturnPlan(rank, world, shift, uniq.to(torch.int32), rowptr.to(torch.int32), enc.to(torch.int32), **extra)
+
+
+# ---- backward of the peer plane: per-slot gradients pulled by the owners of the source rows ------------------------------
+def peer_grad_return_plan(rank: int, world: int, rows: List[torch.Tensor], slots: List[torch.Tensor], n_edges: List[int],
+                          device=None) -> GradReturnPlan:
+    """Owner ``rank``'s reverse slot plan for the peer plane (pure; no communication).
+
+    rows[p]  : int64, this rank's rows (owner-local ids) that the slots of rank p's CSR gather;
+    slots[p] : int64, those slots (ascending), one per entry of rows[p].  The owner's own slots are listed under p = rank;
+    n_edges  : every rank's number of CSR slots.  The position field of ``enc = p << shift | slot`` covers the largest.
+    Each row's slots come out in ascending (rank, slot) order: the slot order of the whole graph's destination-sorted CSR,
+    since the ranks own consecutive destination ranges."""
+    shift = grad_return_shift(max(map(int, n_edges), default=0), world)
+    if device is None:
+        device = rows[0].device if rows else torch.device("cpu")
+    rows_l, enc_l = [], []
+    for p in range(world):
+        ids = rows[p].to(device=device, dtype=torch.int64)
+        if ids.numel() == 0:
+            continue
+        s = slots[p].to(device=device, dtype=torch.int64)
+        if s.numel() != ids.numel():
+            raise ValueError("peer_grad_return_plan: rows and slots differ in length")
+        rows_l.append(ids)
+        enc_l.append((p << shift) | s)
+    return _reverse_csr(rank, world, shift, rows_l, enc_l, device, peer_n_edges=list(map(int, n_edges)))
+
+
+def _slots_by_owner(col: torch.Tensor, shift: int, world: int):
+    """(owner-local rows, slot ids, slots per owner) of one rank's CSR, grouped by owner, slots ascending within an owner."""
+    c = col.to(torch.int64)
+    own = c >> shift
+    order = torch.sort(own, stable=True).indices
+    counts = torch.bincount(own, minlength=world) if c.numel() else torch.zeros(world, dtype=torch.int64, device=c.device)
+    return (c & ((1 << shift) - 1))[order], order, counts
+
+
+def peer_grad_return_plans(cols: List[torch.Tensor], shift: int) -> List[GradReturnPlan]:
+    """Every rank's reverse slot plan from every rank's CSR ``col`` (entries ``owner << shift | row``), in one process
+    (what build_peer_grad_return_plan computes with collectives)."""
+    world = len(cols)
+    segs = [_slots_by_owner(c, shift, world) for c in cols]
+    n_edges = [int(c.numel()) for c in cols]
+    out = []
+    for r in range(world):
+        rows, slots = [], []
+        for p in range(world):
+            rw, sl, counts = segs[p]
+            o = int(counts[:r].sum())
+            c = int(counts[r])
+            rows.append(rw[o:o + c])
+            slots.append(sl[o:o + c])
+        out.append(peer_grad_return_plan(r, world, rows, slots, n_edges, device=cols[r].device))
+    return out
+
+
+def build_peer_grad_return_plan(col: torch.Tensor, shift: int, rank: int, world: int, group=None) -> GradReturnPlan:
+    """This rank's reverse slot plan, once per graph, with two collectives: an all-to-all of (slot count, edge count) per
+    rank pair, then an all-to-all of the (owner-local row, slot) pairs, each rank's grouped by owner."""
+    dev = col.device
+    rows, slots, counts = _slots_by_owner(col, shift, world)
+    meta = torch.stack([counts, torch.full_like(counts, int(col.numel()))], 1)
+    meta_in = torch.empty_like(meta)
+    dist.all_to_all_single(meta_in, meta.contiguous(), group=group)
+    recv = meta_in[:, 0].tolist()
+    pairs = torch.empty((sum(recv), 2), dtype=torch.int64, device=dev)
+    dist.all_to_all_single(pairs, torch.stack([rows, slots], 1).contiguous(), output_split_sizes=recv,
+                           input_split_sizes=counts.tolist(), group=group)
+    got = list(torch.split(pairs, recv))
+    return peer_grad_return_plan(rank, world, [t[:, 0] for t in got], [t[:, 1] for t in got], meta_in[:, 1].tolist(),
+                                 device=dev)
 
 
 def halo_grad_return_plan(plan: HaloPlan) -> GradReturnPlan:
@@ -601,25 +682,102 @@ class PeerAggregator:
     ``x_local`` -- a rank that finishes ``aggregate()`` early must not overwrite its rows while slower peers may still be
     reading them.  Either call ``barrier()`` again after ``aggregate()`` before rewriting ``x_local`` (what a multi-layer net
     using ONE buffer has to do), or alternate between two aggregators / buffers per layer as ``PullAggregator`` does
-    (``flip()``), where the next layer's barrier separates this layer's reads from the writes two layers later."""
+    (``flip()``), where the next layer's barrier separates this layer's reads from the writes two layers later.
+
+    Training (``trainable=True``; opt-in, a forward-only aggregator allocates and communicates nothing more):
+    ``pna_aggregate(x, ...)`` is differentiable in ``x`` and ``row_bias``.  Forward: ``x`` is copied into the next slot of a
+    ring of ``saved_layers`` symmetric row buffers (allocated once, collectively), a device barrier
+    (``pna_peer_barrier``), then the peer forward from that slot's pointer table.  The slot stays readable by the peers until
+    their backward has read it.  Backward, per feature slab (``aggregate.deterministic_slab_width`` of the largest rank's
+    slot count): ``pna_aggregate_bwd_peer_slots`` stores the gradient of every slot of this rank's CSR into its symmetric
+    fp32 per-slot buffer, reading the source rows from the saved slot over NVLink; a barrier; then every owner adds the
+    slots that gather its rows into a zeroed ``[n_local, F]`` gradient with ``pna_halo_grad_pull``, in ascending
+    (rank, slot) order -- the slot order of the whole graph's CSR (``peer_grad_return_plan``).  Rows nobody gathers get zero.
+
+    Reuse.  A rank rewrites a saved slot or a per-slot buffer only after a barrier that no peer enters before its last read
+    of it.  Per-slot buffers alternate (two of them): slab step j+2 rewrites the buffer peers pulled from in step j only
+    after this rank has passed the barrier of step j+1, which no peer enters before its pull of step j is done.  A ring
+    slot written by call i is rewritten by call i + saved_layers, after this rank has passed the barriers of (a) call
+    i + saved_layers - 1 (saved_layers >= 2), which no peer enters before its forward gathers of call i are done, and (b) the
+    last slab of call i's backward, which no peer enters before its backward kernels of call i are done -- provided that
+    backward ran first.  So the caller's rule: every rank makes the same sequence of calls (forward and backward), and at
+    most ``saved_layers`` differentiable calls run between backward passes.  A call beyond that raises, and so does a
+    backward whose saved slot has been rewritten since its forward.
+
+    Determinism: the backward has no floating-point atomic anywhere (per-slot stores, then sums in a fixed order), so it
+    is bit-reproducible whatever ``torch.use_deterministic_algorithms`` says, and it ignores ``PNA_B200_BWD``.  Parameter
+    gradients are this rank's partial sums; summing them across ranks (``all_reduce``) is the caller's job.
+
+    ``_alloc(shape, dtype) -> (local tensor, per-rank pointers, keepalive)`` replaces the symmetric allocation (called for
+    ``x_local``, then, trainable only, the ring slots, the barrier flags and the two per-slot buffers) and ``_barrier`` the
+    device barrier: tests run W ranks in one process through them."""
 
     def __init__(self, src_global: torch.Tensor, dst_global: torch.Tensor, bounds: torch.Tensor, rank: int, world: int,
-                 n_feat: int, dtype=torch.float32, group=None):
+                 n_feat: int, dtype=torch.float32, group=None, trainable: bool = False, saved_layers: int = 2,
+                 grad_plan: Optional[GradReturnPlan] = None, _alloc=None, _barrier=None):
         dev = src_global.device
-        self.rank, self.world, self.group = rank, world, group
+        self.rank, self.world, self.group, self.n_feat, self.dtype = rank, world, group, n_feat, dtype
         lo, hi = int(bounds[rank]), int(bounds[rank + 1])
         self.n_local = hi - lo
         self.shift = peer_shift_for(bounds)
         enc = encode_peer_sources(src_global, bounds, self.shift)
         self.csr = build_csr(enc, dst_global - lo, self.n_local, n_src=world << self.shift)
         rows_max = int((bounds[1:] - bounds[:-1]).max())
-        self.x_local, self.peer_ptrs, self._keep = _symmetric_rows(rows_max, n_feat, dtype, dev, rank, world, group)
+        if _alloc is None:
+            self.x_local, self.peer_ptrs, self._keep = _symmetric_rows(rows_max, n_feat, dtype, dev, rank, world, group)
+            alloc = lambda shape, dt: _symmetric_tensor(shape, dt, dev, rank, world, group)  # noqa: E731
+        else:
+            self.x_local, self.peer_ptrs, self._keep = _alloc((rows_max, n_feat), dtype)
+            alloc = _alloc
         self.x_local = self.x_local[: self.n_local]
         self.ptr_table = torch.tensor(self.peer_ptrs, dtype=torch.int64, device=dev)
+        self.trainable, self.grad_plan = trainable, None
+        if not trainable:
+            return
+        if saved_layers < 2:
+            raise ValueError("saved_layers must be at least 2 (a slot is rewritten only after the next call's barrier)")
+        if grad_plan is None:
+            col = self.csr.col[: self.csr.n_edges]
+            grad_plan = build_peer_grad_return_plan(col, self.shift, rank, world, group) if world > 1 else \
+                peer_grad_return_plan(rank, 1, [col.long() & ((1 << self.shift) - 1)],
+                                      [torch.arange(col.numel(), device=dev)], [col.numel()], device=dev)
+        if grad_plan.rank != rank or grad_plan.world != world:
+            raise ValueError("grad_plan belongs to another rank or world")
+        if grad_plan.peer_n_edges is None or grad_plan.peer_n_edges[rank] != self.csr.n_edges:
+            raise ValueError("grad_plan is not this graph's peer-plane reverse slot plan (peer_grad_return_plan)")
+        self.grad_plan = grad_plan
+        self._ring, self._ring_tables, self._ring_gen, self._ring_keep = [], [], [], []
+        for _ in range(saved_layers):
+            t, ptrs, keep = alloc((rows_max, n_feat), dtype)
+            self._ring.append(t)
+            self._ring_tables.append(torch.tensor(ptrs, dtype=torch.int64, device=dev))
+            self._ring_gen.append(0)
+            self._ring_keep.append(keep)
+        self._next, self._calls_since_backward = 0, 0
+        flags, fptrs, keep = alloc((max(world, 1),), torch.int64)
+        flags.zero_()
+        self._flags, self._flag_table = flags, torch.tensor(fptrs, dtype=torch.int64, device=dev)
+        self._ring_keep.append(keep)
+        self._status = torch.zeros(1, dtype=torch.int32, device=dev)
+        self._epoch = 0
+        # per-slot gradient buffers: the same pitch on every rank (the slab width of the largest rank's slot count)
+        self._e_max = max(max(grad_plan.peer_n_edges), 1)
+        self._slab = deterministic_slab_width(self._e_max, n_feat, 16 // torch.empty(0, dtype=dtype).element_size())
+        self._gbufs, self._gtables, self._gcur = [], [], 0
+        for _ in range(2):
+            t, ptrs, keep = alloc((self._e_max, self._slab), torch.float32)
+            self._gbufs.append(t)
+            self._gtables.append(torch.tensor(ptrs, dtype=torch.int64, device=dev))
+            self._ring_keep.append(keep)
+        self._barrier_hook = _barrier
+        self._use_device_barrier = _barrier is None and (world > 1 and _alloc is None)
+        if self._use_device_barrier:      # flags are zero everywhere before the first flag store can arrive
+            torch.cuda.synchronize(dev)
+            dist.barrier(group=group, device_ids=[dev.index])
 
     def barrier(self) -> None:
         """All ranks have finished writing their x rows (device-side, on the current stream)."""
-        h = self._keep.get("handle")
+        h = self._keep.get("handle") if isinstance(self._keep, dict) else None
         if h is not None and hasattr(h, "barrier"):
             h.barrier()
         else:
@@ -628,6 +786,144 @@ class PeerAggregator:
     def aggregate(self, aggregators, scalers, avg_deg, out: Optional[torch.Tensor] = None, **kw) -> torch.Tensor:
         return aggregate_forward(self.x_local, self.csr, aggregators, scalers, avg_deg, out=out,
                                  peer=(self.ptr_table, self.shift), **kw)
+
+    # ---- differentiable path (trainable=True) ----
+    def _sync(self) -> None:
+        """The trainable path's barrier: ``pna_peer_barrier`` on the current stream (or the ``_barrier`` hook)."""
+        if self._barrier_hook is not None:
+            self._barrier_hook()
+            return
+        if not self._use_device_barrier:
+            return
+        self._epoch += 1
+        dev = self._flags.device
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().pna_peer_barrier(self._flag_table.data_ptr(), self.rank, self.world, self._epoch, 0,
+                                                   self._status.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+
+    def check(self) -> None:
+        """Host-side check (synchronises): did every barrier of the trainable path see all peers arrive?"""
+        if self.trainable and int(self._status.item()) != 0:
+            raise RuntimeError("pna_peer_barrier timed out: a peer rank did not reach the barrier")
+
+    def pna_aggregate(self, x: torch.Tensor, aggregators, scalers, avg_deg, *, towers: int = 1,
+                      row_bias: Optional[torch.Tensor] = None, self_feat: Optional[torch.Tensor] = None,
+                      self_divided: bool = True, zero_isolated: bool = False, relu_var: bool = False,
+                      scaler_degree: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Differentiable aggregation of this rank's rows, gathered over NVLink: x is the rank's ``[n_local, F]``
+        features, ``row_bias`` / ``self_feat`` are per destination and stay local; returns the rank's ``[n_local, width]``
+        output.  Needs ``trainable=True``; the rules on the call sequence are in the class docstring."""
+        if not self.trainable:
+            raise RuntimeError("PeerAggregator.pna_aggregate needs PeerAggregator(..., trainable=True)")
+        if tuple(x.shape) != (self.n_local, self.n_feat) or x.dtype != self.dtype:
+            raise ValueError(f"x must be [{self.n_local}, {self.n_feat}] {self.dtype}, got {tuple(x.shape)} {x.dtype}")
+        if any(a in _lib.MOMENTS + _lib.WEIGHTED for a in _names(aggregators)):
+            raise ValueError("the peer plane has no moment, softmax, softmin or normalised_mean aggregators")
+        needs_grad = torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x, row_bias, self_feat))
+        if needs_grad and self._calls_since_backward >= len(self._ring):
+            raise RuntimeError(f"more than saved_layers={len(self._ring)} differentiable calls before a backward: the "
+                               "oldest saved features would be overwritten")
+        slot = self._next
+        self._next = (slot + 1) % len(self._ring)
+        self._ring_gen[slot] += 1
+        self._ring[slot][: self.n_local].copy_(x)
+        self._sync()
+        kw = dict(towers=towers, self_divided=self_divided, zero_isolated=zero_isolated, relu_var=relu_var,
+                  scaler_degree=scaler_degree)
+        if not needs_grad:
+            return self._aggregate_saved(slot, aggregators, scalers, avg_deg, row_bias, self_feat, kw)
+        self._calls_since_backward += 1
+        return _PeerAggregate.apply(x, row_bias, self_feat, self, slot, _names(aggregators), _names(scalers), dict(avg_deg), kw)
+
+    def _aggregate_saved(self, slot: int, aggregators, scalers, avg_deg, row_bias, self_feat, kw) -> torch.Tensor:
+        return aggregate_forward(self._ring[slot][: self.n_local], self.csr, aggregators, scalers, avg_deg,
+                                 row_bias=row_bias, self_feat=self_feat, peer=(self._ring_tables[slot], self.shift), **kw)
+
+    def _backward_slots(self, grad_out: torch.Tensor, slot: int, aggregators, scalers, avg_deg, *, towers: int = 1,
+                       row_bias: Optional[torch.Tensor] = None, has_self: bool = False, relu_var: bool = False,
+                       scaler_degree: Optional[torch.Tensor] = None, need_bias_grad: bool = False):
+        """The backward of the forward run from ring slot ``slot``: (fp32 gradient of this rank's x, fp32 gradient of
+        row_bias or None).  Collective: every rank runs it for the same call, in the same order."""
+        n, F, csr = self.n_local, self.n_feat, self.csr
+        dev = self._ring[slot].device
+        x = self._ring[slot][:n]
+        n_aggr, aggr_codes = _lib.pack_codes(aggregators, _lib.ALL_AGGR_CODES, "aggregator")
+        n_scal, scal_codes = _lib.pack_codes(scalers, _lib.SCALER_CODES, "scaler")
+        grad_out = _rows2d(grad_out.to(self.dtype), "grad_out")
+        if row_bias is not None:
+            row_bias = _rows2d(row_bias.to(self.dtype), "row_bias")
+        gb = torch.zeros((n, F), dtype=torch.float32, device=dev) if need_bias_grad else None
+        d = _lib.AggStruct(
+            gathered=x.data_ptr(), ld_gathered=F, rowptr=csr.rowptr.data_ptr(), col=csr.col.data_ptr() if csr.n_edges else None,
+            row_bias=None if row_bias is None else row_bias.data_ptr(),
+            ld_row_bias=0 if row_bias is None else (row_bias.stride(0) if n > 1 else F),
+            self_feat=1 if has_self else None,     # only its presence matters here: it shifts the grad_out columns
+            n_rows=n, n_feat=F, n_towers=towers, dtype=_DTYPES[self.dtype],
+            n_aggr=n_aggr, aggr_codes=aggr_codes, n_scalers=n_scal, scaler_codes=scal_codes,
+            avg_log=float(avg_deg["log"]), avg_lin=float(avg_deg.get("lin", 1.0)),
+            flags=_lib.FLAG_RELU_VAR if relu_var else 0, split_threshold=csr.split_threshold, chunk_edges=csr.chunk_edges,
+            hub_info=csr.hub_info.data_ptr() if csr.n_hubs else None,
+            chunk_items=csr.chunk_items.data_ptr() if csr.n_hubs else None, n_hubs=csr.n_hubs, n_chunks=csr.n_chunks,
+            peer_gathered=self._ring_tables[slot].data_ptr(), peer_shift=self.shift)
+        if scaler_degree is not None:
+            d.scaler_degree = scaler_degree.data_ptr()
+        scratch = None
+        if csr.n_hubs:
+            scratch = torch.empty(((csr.n_chunks + csr.n_hubs) * 6, F), dtype=torch.float32, device=dev)
+            d.hub_partials = scratch.data_ptr()
+        ld_go = grad_out.stride(0) if n > 1 else grad_out.size(1)
+        gp, L = self.grad_plan, _lib.lib()
+        g = torch.zeros((n, F), dtype=torch.float32, device=dev)
+        for f0 in range(0, F, self._slab):
+            fc = min(self._slab, F - f0)
+            gs = self._gbufs[self._gcur].view(-1)[: self._e_max * fc].view(self._e_max, fc)
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            if csr.n_edges:
+                with torch.cuda.device(dev):
+                    _lib.check(L.pna_aggregate_bwd_peer_slots(C.byref(d), grad_out.data_ptr(), ld_go, f0, fc, gs.data_ptr(), fc,
+                                                              None if gb is None else gb.data_ptr(), F, stream))
+            self._sync()          # every rank's per-slot gradients of this slab are stored
+            if gp.n_rows:
+                with torch.cuda.device(dev):
+                    _lib.check(L.pna_halo_grad_pull(self._gtables[self._gcur].data_ptr(), fc, gp.rows.data_ptr(),
+                                                    gp.rowptr.data_ptr(), gp.enc.data_ptr(), gp.shift, gp.n_rows,
+                                                    g[:, f0:].data_ptr(), F, fc, stream))
+            self._gcur = (self._gcur + 1) % len(self._gbufs)
+        return g, gb
+
+
+class _PeerAggregate(torch.autograd.Function):
+    """The peer plane's differentiable aggregation (``PeerAggregator.pna_aggregate``): x lives in a ring slot of the
+    aggregator, which the backward reads through the peers' pointer table."""
+
+    @staticmethod
+    def forward(ctx, x, row_bias, self_feat, agg, slot, aggregators, scalers, avg_deg, kw):
+        out = agg._aggregate_saved(slot, aggregators, scalers, avg_deg, row_bias, self_feat, kw)
+        ctx.save_for_backward(row_bias, self_feat)
+        ctx.meta = (agg, slot, agg._ring_gen[slot], aggregators, scalers, avg_deg, kw, x.dtype)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        row_bias, self_feat = ctx.saved_tensors
+        agg, slot, gen, aggregators, scalers, avg_deg, kw, x_dtype = ctx.meta
+        if agg._ring_gen[slot] != gen:
+            raise RuntimeError("the saved features of this peer-plane call were overwritten by a later call before its "
+                               f"backward: at most saved_layers={len(agg._ring)} differentiable calls between backward passes")
+        agg._calls_since_backward = 0
+        towers = kw["towers"]
+        g, gb = agg._backward_slots(grad_out, slot, aggregators, scalers, avg_deg, towers=towers, row_bias=row_bias,
+                                   has_self=self_feat is not None, relu_var=kw["relu_var"],
+                                   scaler_degree=kw["scaler_degree"], need_bias_grad=ctx.needs_input_grad[1])
+        gs = None
+        if self_feat is not None and ctx.needs_input_grad[2]:
+            # the self block of every tower is a plain copy: its gradient is the matching slice of grad_out
+            N, F = agg.n_local, agg.n_feat
+            Ft = F // towers
+            blk = grad_out.reshape(N, towers, -1)[:, :, :Ft]
+            gs = (blk.reshape(N, F) if kw["self_divided"] else blk.sum(1)).to(self_feat.dtype)
+        return (g.to(x_dtype) if ctx.needs_input_grad[0] else None, None if gb is None else gb.to(row_bias.dtype), gs,
+                None, None, None, None, None, None)
 
 
 def _symmetric_rows(rows: int, n_feat: int, dtype, dev, rank: int, world: int, group):

@@ -1,5 +1,5 @@
 """torchrun --nproc-per-node N tools/dist_check.py : multi-GPU parity of the peer, halo and pull paths against the oracle,
-and of the pull and halo paths' backward (the gradient returned to every rank's rows) against the oracle's autograd."""
+and of the pull, halo and peer paths' backward (the gradient returned to every rank's rows) against the oracle's autograd."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch, torch.distributed as dist
@@ -69,6 +69,18 @@ for (n, e, f, hubdeg) in [(4000, 40000, 128, 3000), (3000, 20000, 64, 0), (5000,
     ok &= good
     print(f"rank {rank} n={n} f={f} halo backward: max err {(gh - gw).abs().max().item():.2e} "
           f"return rows={halo.grad_plan.n_rows} {'ok' if good else 'MISMATCH'}", flush=True)
+    # peer path, forward and backward: per-slot gradients read over NVLink, pulled back by the sources' owners
+    peer = pd.PeerAggregator(src[mine].to(dev), dst[mine].to(dev), bounds, rank, world, f, trainable=True)
+    xp = x[lo:hi].to(dev).requires_grad_(True)
+    outp = peer.pna_aggregate(xp, A4, S3, avg)
+    (outp * w[lo:hi].to(dev)).sum().backward()
+    peer.check()
+    check(outp.detach(), "peer differentiable")
+    gp = xp.grad.cpu()
+    good = torch.allclose(gp, gw, rtol=1e-3, atol=5e-4)
+    ok &= good
+    print(f"rank {rank} n={n} f={f} peer backward: max err {(gp - gw).abs().max().item():.2e} "
+          f"return rows={peer.grad_plan.n_rows} {'ok' if good else 'MISMATCH'}", flush=True)
     torch.cuda.synchronize(); dist.barrier(device_ids=[local])
 t = torch.tensor([1 if ok else 0], device=dev); dist.all_reduce(t, op=dist.ReduceOp.MIN)
 if rank == 0: print("DIST ALL OK" if int(t) else "DIST FAILED")
