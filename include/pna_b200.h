@@ -352,6 +352,19 @@ int pna_edge_msg_fwd(const int32_t* rowptr, const int32_t* col, int64_t n_rows, 
 int pna_edge_msg_bwd(const float* grad_messages, int32_t msg_pitch, const float* activations, const float* weight,
                      int64_t n_edges, int32_t n_layers, int32_t n_towers, int32_t width, float* grad_pre, pna_stream_t stream);
 
+/* The same two calls with bf16 storage (the layers under bf16 autocast).  a, b, edge_term, messages, activations and
+ * grad_messages are bf16 (const void* / void*: 2-byte elements, same layouts and pitches); bias1, weight, bias and grad_pre
+ * stay fp32.  A load widens to fp32 exactly and the arithmetic is the fp32 calls', so bit for bit
+ *     messages_bf16 = RN_bf16(pna_edge_msg_fwd(a, b, edge_term widened)),   activations likewise,
+ *     grad_pre      = pna_edge_msg_bwd(grad_messages widened, activations widened)   (ReLU mask: stored z > 0).
+ * Same arguments, checks and status codes as the fp32 calls.  (Appended in ABI version 8.) */
+int pna_edge_msg_fwd_bf16(const int32_t* rowptr, const int32_t* col, int64_t n_rows, int64_t n_edges, const void* a, const void* b,
+                          const float* bias1, const void* edge_term, const float* weight, const float* bias, int32_t n_layers,
+                          int32_t n_towers, int32_t width, int32_t msg_pitch, void* messages, void* activations,
+                          pna_stream_t stream);
+int pna_edge_msg_bwd_bf16(const void* grad_messages, int32_t msg_pitch, const void* activations, const float* weight,
+                          int64_t n_edges, int32_t n_layers, int32_t n_towers, int32_t width, float* grad_pre, pna_stream_t stream);
+
 /* ---- halo rows for the destination-partitioned multi-GPU path (north_star: "single NCCL all-to-all for halo
  * source features per layer"): dst[i, :] = src[idx[i], :], n_feat elements per row.  Used to pack the send buffer. */
 int pna_gather_rows(const void* src, int64_t ld_src, const int32_t* idx, int64_t n_idx, void* dst, int64_t ld_dst,
@@ -462,6 +475,13 @@ int pna_linear_towers_scaled_fwd(const float* a, int64_t lda, const float* row_s
 int pna_linear_towers_bwd_data(const float* grad_y, int64_t ld_grad_y, const float* row_scale, int32_t n_scalers, const float* weight,
                                float* grad_a, int64_t ld_grad_a, int64_t n_rows, int32_t n_towers, int32_t n_feat, int32_t n_aggr,
                                int32_t n_out, pna_stream_t stream);
+/* pna_linear_towers_scaled_fwd with a bf16 compact aggregate `a` (const void*: 2-byte elements, pitch lda in elements);
+ * row_scale, weight, bias and y stay fp32.  Each element of a is widened to fp32 (exact) as it is loaded; from there on
+ * the arithmetic is the fp32 call's, so y equals pna_linear_towers_scaled_fwd(a widened) bit for bit.  Same checks and
+ * status codes.  The data gradient needs no bf16 call: grad_y is fp32.  (Appended in ABI version 8.) */
+int pna_linear_towers_scaled_fwd_bf16(const void* a, int64_t lda, const float* row_scale, int32_t n_scalers, const float* weight,
+                                      const float* bias, float* y, int64_t ldy, int64_t n_rows, int32_t n_towers, int32_t n_feat,
+                                      int32_t n_aggr, int32_t n_out, pna_stream_t stream);
 
 int pna_query(int what);
 const char* pna_last_error(void);

@@ -51,7 +51,8 @@ EXPORTED_SYMBOLS = ("pna_csr_workspace_bytes", "pna_csr_build", "pna_csr_light_v
                     "pna_gather_rows", "pna_halo_pull", "pna_halo_grad_pull", "pna_peer_barrier", "pna_linear_fwd", "pna_linear_scaled_fwd", "pna_row_scales", "pna_linear_workspace_bytes",
                     "pna_linear_bwd_workspace_bytes", "pna_linear_bwd_data", "pna_linear_bwd_weight", "pna_edge_mlp_fwd",
                     "pna_edge_mlp_bwd", "pna_edge_msg_fwd", "pna_edge_msg_bwd", "pna_query", "pna_last_error",
-                    "pna_linear_towers_scaled_fwd", "pna_linear_towers_bwd_data")
+                    "pna_linear_towers_scaled_fwd", "pna_linear_towers_bwd_data", "pna_edge_msg_fwd_bf16", "pna_edge_msg_bwd_bf16",
+                    "pna_linear_towers_scaled_fwd_bf16")
 
 
 class PnaError(RuntimeError):
@@ -231,6 +232,12 @@ def lib() -> C.CDLL:
         L.pna_linear_towers_bwd_data.restype = C.c_int
         L.pna_linear_towers_bwd_data.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64,
                                                  C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
+        L.pna_edge_msg_fwd_bf16.restype = C.c_int
+        L.pna_edge_msg_fwd_bf16.argtypes = L.pna_edge_msg_fwd.argtypes
+        L.pna_edge_msg_bwd_bf16.restype = C.c_int
+        L.pna_edge_msg_bwd_bf16.argtypes = L.pna_edge_msg_bwd.argtypes
+        L.pna_linear_towers_scaled_fwd_bf16.restype = C.c_int
+        L.pna_linear_towers_scaled_fwd_bf16.argtypes = L.pna_linear_towers_scaled_fwd.argtypes
         abi = L.pna_query(QUERY_ABI_VERSION)
         if abi != ABI_VERSION:
             raise ImportError(f"{LIB_PATH} has ABI version {abi}, this package needs {ABI_VERSION}: rebuild it")

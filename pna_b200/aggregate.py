@@ -68,6 +68,29 @@ def fold_finalize_enabled() -> bool:
     return os.environ.get("PNA_B200_FOLD_FINALIZE", "0") == "1"
 
 
+def boundary_dtype() -> Optional[torch.dtype]:
+    """The one rule for mixed precision (DESIGN section 2): the dtype in which the layers hand the products of their node
+    and edge GEMMs to the kernels inside a CUDA ``torch.autocast`` region.
+
+    * bf16 autocast: ``torch.bfloat16``.  U / V, A / Bm / C and the messages stay as autocast made them and go to the bf16
+      kernel instances (aggregation, per-edge messages, compact tower post-linear); the weights stay fp32.
+    * any other autocast dtype (float16): ``torch.float32``.  There are no fp16 kernel instances, so fp16 operands are
+      upcast (``at_boundary``) and run the fp32 kernels.
+    * no autocast: ``None`` -- the layers decide on the tensors' own dtypes, as they always have.
+    Every layer asks this function (as ``aggregate.boundary_dtype()``), so it is the one place autocast is read."""
+    if not torch.is_autocast_enabled("cuda"):
+        return None
+    return torch.bfloat16 if torch.get_autocast_dtype("cuda") == torch.bfloat16 else torch.float32
+
+
+def at_boundary(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
+    """A kernel operand made inside an autocast region, at the kernel boundary: float16 is upcast to float32 (no fp16
+    kernels); every other tensor, and every tensor outside autocast, passes as it is."""
+    if t is not None and t.dtype == torch.float16 and boundary_dtype() is not None:
+        return t.float()
+    return t
+
+
 def output_width(n_feat: int, n_aggr: int, n_scalers: int, has_self: bool) -> int:
     return (n_aggr * n_scalers + (1 if has_self else 0)) * n_feat
 

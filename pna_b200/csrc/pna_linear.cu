@@ -29,6 +29,7 @@
 // Backward -- pna_linear_bwd_data / pna_linear_bwd_weight, at the same fp32 accuracy and deterministic (no atomics):
 // dA runs the kernel above on dY with the transposed weight in column slabs; dW is k_linear_bwd_weight (below).
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -655,11 +656,17 @@ struct TwrSmem {
   static constexpr size_t kBytes = 1024 /*align slack*/ + (size_t)kTwrSt * kStage;
 };
 
-template <bool BWD>
-__global__ void __launch_bounds__(kLinThreads, 1)
-k_towers_3xtf32(const float* __restrict__ X, long long ldx, const float* __restrict__ row_scale, int S,
-                const float* __restrict__ W, const float* __restrict__ bias, float* __restrict__ Y, long long ldy, long long N,
-                int T, int Fp, int AF, int Ot, int n_slabs) {
+// X's element: fp32, or bf16 (the forward under bf16 autocast) widened to fp32 on load, which is exact; everything after the
+// load is the fp32 kernel's, so the bf16 instance computes what the fp32 one computes on the widened aggregate
+__device__ __forceinline__ float twr_ld(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float twr_ld(const __nv_bfloat16* p) {
+  return __uint_as_float(static_cast<unsigned>(__ldg(reinterpret_cast<const unsigned short*>(p))) << 16);
+}
+
+template <bool BWD, typename TX>
+__device__ __forceinline__ void towers_3xtf32(const TX* __restrict__ X, long long ldx, const float* __restrict__ row_scale, int S,
+                                              const float* __restrict__ W, const float* __restrict__ bias, float* __restrict__ Y,
+                                              long long ldy, long long N, int T, int Fp, int AF, int Ot, int n_slabs) {
   extern __shared__ unsigned char lin_raw[];
   const unsigned base = (lin_smem_u32(lin_raw) + 1023u) & ~1023u;
   unsigned char* gbase = lin_raw + (base - lin_smem_u32(lin_raw));
@@ -698,7 +705,7 @@ k_towers_3xtf32(const float* __restrict__ X, long long ldx, const float* __restr
       for (int sl = 0; sl < kSlabs; ++sl) {
         const long long r = row0 + sl * 32 + r_in;
         const bool ok = live && r < N;
-        xa[sl][e] = ok ? __ldg(X + r * ldx + col) : 0.f;
+        xa[sl][e] = ok ? twr_ld(X + r * ldx + col) : 0.f;
         xs[sl][e] = (ok && s >= 0) ? __ldg(row_scale + r * S + s) : 1.f;
       }
     }
@@ -808,9 +815,28 @@ k_towers_3xtf32(const float* __restrict__ X, long long ldx, const float* __restr
 }
 
 template <bool BWD>
-static int launch_towers(const float* X, long long ldx, const float* row_scale, int S, const float* W, const float* bias, float* Y,
+__global__ void __launch_bounds__(kLinThreads, 1)
+k_towers_3xtf32(const float* __restrict__ X, long long ldx, const float* __restrict__ row_scale, int S,
+                const float* __restrict__ W, const float* __restrict__ bias, float* __restrict__ Y, long long ldy, long long N,
+                int T, int Fp, int AF, int Ot, int n_slabs) {
+  towers_3xtf32<BWD, float>(X, ldx, row_scale, S, W, bias, Y, ldy, N, T, Fp, AF, Ot, n_slabs);
+}
+
+// the forward on a bf16 compact aggregate (pna_linear_towers_scaled_fwd_bf16)
+__global__ void __launch_bounds__(kLinThreads, 1)
+k_towers_bf16_3xtf32(const __nv_bfloat16* __restrict__ X, long long ldx, const float* __restrict__ row_scale, int S,
+                     const float* __restrict__ W, const float* __restrict__ bias, float* __restrict__ Y, long long ldy, long long N,
+                     int T, int Fp, int AF, int Ot, int n_slabs) {
+  towers_3xtf32<false, __nv_bfloat16>(X, ldx, row_scale, S, W, bias, Y, ldy, N, T, Fp, AF, Ot, n_slabs);
+}
+
+template <bool BWD, typename TX = float>
+static int launch_towers(const TX* X, long long ldx, const float* row_scale, int S, const float* W, const float* bias, float* Y,
                          long long ldy, long long N, int T, int Fp, int AF, int Ot, cudaStream_t st) {
-  auto kern = k_towers_3xtf32<BWD>;
+  void (*kern)(const TX*, long long, const float*, int, const float*, const float*, float*, long long, long long, int, int, int, int,
+               int);
+  if constexpr (std::is_same<TX, float>::value) kern = k_towers_3xtf32<BWD>;
+  else kern = k_towers_bf16_3xtf32;
   static bool attr_set = false;
   if (!attr_set) {
     PNA_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TwrSmem::kBytes));
@@ -980,6 +1006,20 @@ extern "C" int pna_linear_towers_scaled_fwd(const float* a, int64_t lda, const f
               "%s: row pitch smaller than the row", who);
   return launch_towers<false>(a, lda, row_scale, n_scalers, weight, bias, y, ldy, n_rows, n_towers, n_feat, n_aggr * n_feat, n_out,
                               static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int pna_linear_towers_scaled_fwd_bf16(const void* a, int64_t lda, const float* row_scale, int32_t n_scalers,
+                                                 const float* weight, const float* bias, float* y, int64_t ldy, int64_t n_rows,
+                                                 int32_t n_towers, int32_t n_feat, int32_t n_aggr, int32_t n_out, pna_stream_t stream) {
+  const char* who = "pna_linear_towers_scaled_fwd_bf16";
+  const int rc = towers_check(n_rows, n_towers, n_feat, n_aggr, n_out, n_scalers, who);
+  if (rc != PNA_OK) return rc;
+  if (n_rows == 0) return PNA_OK;
+  PNA_REQUIRE(a && row_scale && weight && y, PNA_ERR_BAD_ARG, "%s: null pointer", who);
+  PNA_REQUIRE(lda >= (int64_t)n_towers * (1 + n_aggr) * n_feat && ldy >= (int64_t)n_towers * n_out, PNA_ERR_BAD_ARG,
+              "%s: row pitch smaller than the row", who);
+  return launch_towers<false>(static_cast<const __nv_bfloat16*>(a), lda, row_scale, n_scalers, weight, bias, y, ldy, n_rows, n_towers,
+                              n_feat, n_aggr * n_feat, n_out, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int pna_linear_towers_bwd_data(const float* grad_y, int64_t ld_grad_y, const float* row_scale, int32_t n_scalers,

@@ -36,13 +36,15 @@ edge of the row CSR, writing M [E, T*F_t] in slot order.  The self-first aggrega
 with ``degree_col = row.col``); max/min read the same messages through a third CSR (destination j, sources = the row-slot
 ids of the edges (i, j)), because X[u, v] of the colwise reduction is the message of edge (u, v); ``identity`` runs the
 pretrans MLP on [h_i, h_i] in torch.  Tower widths above 64 raise NotImplementedError.
+Under ``torch.autocast("cuda")`` A and Bm reach the kernel at the boundary (DESIGN section 2): bf16 ones run
+``pna_edge_msg_fwd_bf16`` (no edge term, pitch F_t: the arithmetic of ``pna_edge_mlp_fwd``), fp16 ones are upcast to fp32.
 """
 from __future__ import annotations
 
 import torch
 import torch.nn as nn
 
-from .aggregate import aggregate_forward, pna_aggregate
+from .aggregate import aggregate_forward, at_boundary, pna_aggregate
 from .csr import build_csr, tensor_version
 from .edge_mlp import edge_mlp
 from . import _lib
@@ -205,6 +207,7 @@ class PNALayer(nn.Module):
         if not all(tw.pretrans.is_linear_relu() for tw in self.towers):
             raise NotImplementedError("dense PNALayer: the edge-MLP kernel takes Linear/ReLU pretrans layers only")
         A, Bm, b1 = self._halves(h)
+        A, Bm = at_boundary(A), at_boundary(Bm)
         W = torch.stack([torch.stack([fcs[k].linear.weight for fcs in mlps]) for k in range(1, len(mlps[0]))])
         bW = torch.stack([torch.stack([fcs[k].linear.bias for fcs in mlps]) for k in range(1, len(mlps[0]))])
         M = edge_mlp(A, Bm, b1, W, bW, graphs.row, T)

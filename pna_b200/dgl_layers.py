@@ -14,6 +14,10 @@ pretrans layer they are affine and never built (two node GEMMs and the aggregati
 torch on gathered rows only for inputs the kernel does not take: dtypes other than float32, ``pretrans_layers > 1`` with
 a tower width above 64, pretrans stacks that are not plain Linear / ReLU (dropout or batch norm inside), and training
 steps on graphs below ``edge_mlp.FUSED_TRAINING_MIN_EDGES`` edges, where the torch path measured faster.
+
+Under ``torch.autocast("cuda")`` ``PNALayer`` hands its GEMM products to the kernels in ``aggregate.boundary_dtype()``
+(DESIGN section 2): bf16 operands run the bf16 aggregation, messages and compact tower post-linear whatever h's dtype, fp16
+ones are upcast to fp32.  The tower width is padded for that dtype; the weights stay fp32.
 """
 from __future__ import annotations
 
@@ -21,8 +25,8 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import _lib, padding as pad
-from .aggregate import pna_aggregate, row_scales
+from . import _lib, aggregate, padding as pad
+from .aggregate import at_boundary, pna_aggregate, row_scales
 from . import edge_mlp
 from .edge_mlp import edge_messages
 from .linear import compact_path_ok, post_linear_towers_scaled, towers_compact_pays, towers_path_ok
@@ -146,10 +150,13 @@ class PNALayer(nn.Module):
     def _fused_messages_ok(self, h, e, n_edges: int) -> bool:
         """The inputs pna_edge_msg_fwd takes: float32 on the GPU, Linear/ReLU pretrans stacks, and a tower width of at
         most 64 when there is more than one pretrans layer; with autograd, graphs of at least
-        edge_mlp.FUSED_TRAINING_MIN_EDGES edges (where the kernel path is faster)."""
+        edge_mlp.FUSED_TRAINING_MIN_EDGES edges (where the kernel path is faster).  Inside autocast the GEMMs make the
+        operands, in the boundary dtype: the dtypes of h and e are not asked, the weights' is."""
         fc0 = self.towers[0].pretrans.fully_connected
-        return (edge_mlp.fused_step_pays(n_edges) and h.is_cuda and h.dtype == torch.float32 and fc0[0].linear.weight.dtype == torch.float32
-                and (not self.edge_features or (e is not None and e.dtype == torch.float32))
+        amp = aggregate.boundary_dtype() is not None
+        return (edge_mlp.fused_step_pays(n_edges) and h.is_cuda and (amp or h.dtype == torch.float32)
+                and fc0[0].linear.weight.dtype == torch.float32
+                and (not self.edge_features or (e is not None and (amp or e.dtype == torch.float32)))
                 and all(tw.pretrans.is_linear_relu() for tw in self.towers)
                 and (len(fc0) == 1 or self.input_tower <= _lib.EDGE_MLP_MAX_WIDTH))
 
@@ -158,8 +165,9 @@ class PNALayer(nn.Module):
         (source side), A = h W[:, it:2it]^T (destination side), block-diagonal under divide_input; C = ef[perm] W_e^T with
         W_e every tower's W[:, 2it:] stacked (ef is not split by divide_input); the hidden Linears as [L-1, T, it, it]."""
         Wd, Ws, b1, We, W, bW = self._message_weights()
-        C = e.index_select(0, csr.perm.long()) @ We.t() if self.edge_features else None
-        return edge_messages(h @ Wd.t(), h @ Ws.t(), b1, W, bW, csr, len(self.towers), edge_term=C, pitch=fp)
+        C = at_boundary(e.index_select(0, csr.perm.long()) @ We.t()) if self.edge_features else None
+        return edge_messages(at_boundary(h @ Wd.t()), at_boundary(h @ Ws.t()), b1, W, bW, csr, len(self.towers), edge_term=C,
+                             pitch=fp)
 
     def _message_weights(self):
         """The pretrans weights packed as the kernel takes them; rebuilt only when a parameter changed (without autograd;
@@ -216,7 +224,7 @@ class PNALayer(nn.Module):
         h_in = h
         csr = graph_csr(g, h.device)
         T, it = len(self.towers), self.input_tower
-        fp = pad.padded_width(it, h.dtype)
+        fp = pad.padded_width(it, aggregate.boundary_dtype() or h.dtype)      # the kernels' dtype: bf16 pads to 8 columns
         if fp == it:
             h_self = h
         elif self.divide_input:
@@ -227,13 +235,13 @@ class PNALayer(nn.Module):
         compact = self._compact(h, fp)
         scalers = ["identity"] if compact else self.scalers
         if not self.edge_features and self.towers[0].pretrans.is_single_affine():
-            U, V = self._affine_terms(h, fp)
+            U, V = (at_boundary(t) for t in self._affine_terms(h, fp))
             agg = pna_aggregate(V, csr, self.aggregators, scalers, self.avg_d, row_bias=U, **common)
         else:
             if self._fused_messages_ok(h, e, csr.n_edges):
                 msgs = self._fused_messages(csr, h, e, fp)
             else:
-                msgs = pad.pad_blocks(self._edge_messages(csr, h, e), T, it, fp)
+                msgs = at_boundary(pad.pad_blocks(self._edge_messages(csr, h, e), T, it, fp))
             agg = pna_aggregate(msgs, csr, self.aggregators, scalers, self.avg_d, messages_in_csr_order=True, **common)
         blocks = 1 + len(self.aggregators) * len(self.scalers)
         if compact:

@@ -14,6 +14,11 @@ gradients are library GEMMs and sums (as ``linear.library_grad_weight``), and ``
 ``pna_edge_msg_bwd``): the edge-feature columns of the first layer arrive as one per-slot term ``C`` (a single GEMM over
 the permuted edge features), any ``L >= 1`` is taken (``L = 1``: the message is the first layer's output, any width), and
 the messages are written at the aggregation's padded tower pitch, pad columns zero, so no copy follows.
+
+bf16 operands (the layers under bf16 autocast, DESIGN section 2): ``edge_messages`` and ``edge_mlp`` take A, Bm and C in
+bfloat16 with fp32 weights and run ``pna_edge_msg_fwd_bf16`` / ``pna_edge_msg_bwd_bf16``: the messages and the stored
+activations are bf16, the pre-activation gradients fp32; the result is the fp32 kernel's on the widened operands, rounded
+to bf16 once.  Explicit bf16 models (bf16 weights) are not taken: the fp32-weight rule keeps them on their torch path.
 """
 from __future__ import annotations
 
@@ -116,7 +121,11 @@ def _first_layer_grads(ctx, G1, csr: CSRGraph, n_src: int):
 
 def edge_mlp(A, Bm, b1, W, bW, csr: CSRGraph, towers: int) -> torch.Tensor:
     """Differentiable per-edge MLP messages ``[E, T*F_t]`` in slot order of ``csr``:
-    ``M[s, t] = W_L[t] relu(... relu(A[i, t] + Bm[col[s], t] + b1[t]) ...) + b_L[t]`` (see include/pna_b200.h)."""
+    ``M[s, t] = W_L[t] relu(... relu(A[i, t] + Bm[col[s], t] + b1[t]) ...) + b_L[t]`` (see include/pna_b200.h).
+    bf16 A / Bm with fp32 weights (bf16 autocast) take ``edge_messages`` without edge term at pitch F_t: the same
+    arithmetic (DESIGN section 2), with bf16 storage."""
+    if A.dtype == torch.bfloat16 and W.dtype == torch.float32:
+        return edge_messages(A, Bm, b1, W, bW, csr, towers)
     if torch.is_grad_enabled() and any(t.requires_grad for t in (A, Bm, b1, W, bW)):
         return _EdgeMLP.apply(A, Bm, b1, W, bW, csr, towers)
     return edge_mlp_forward(A, Bm, b1, W, bW, csr, towers)[0]
@@ -141,39 +150,49 @@ def _check_messages(A, Bm, b1, W, bW, csr: CSRGraph, towers: int, edge_term, pit
     if P < Ft:
         raise ValueError(f"edge messages: pitch {P} < tower width {Ft}")
     for t in (A, Bm, b1, edge_term) + ((W, bW) if L > 1 else ()):
-        if t is not None and (t.dtype != torch.float32 or not t.is_cuda):
-            raise TypeError("the edge message kernel takes float32 CUDA tensors")
+        if t is not None and not t.is_cuda:
+            raise TypeError("the edge message kernel takes CUDA tensors")
+    if A.dtype not in _KERNEL or any(t is not None and t.dtype != A.dtype for t in (Bm, edge_term)):
+        raise TypeError("the edge message kernel takes A, Bm and edge_term in one dtype, float32 or bfloat16")
+    if any(t.dtype != torch.float32 for t in (b1,) + ((W, bW) if L > 1 else ())):
+        raise TypeError("the edge message kernel takes float32 biases and weights")
     if L > 1 and Ft > _lib.EDGE_MLP_MAX_WIDTH:
         raise NotImplementedError(f"edge messages: tower width {Ft} > {_lib.EDGE_MLP_MAX_WIDTH} with {L} layers is not "
                                   "supported by pna_edge_msg_fwd")
     return L, T, Ft, P
 
 
+# the entry points per storage dtype of A / Bm / C, the messages and the activations
+_KERNEL = {torch.float32: ("pna_edge_msg_fwd", "pna_edge_msg_bwd"),
+           torch.bfloat16: ("pna_edge_msg_fwd_bf16", "pna_edge_msg_bwd_bf16")}
+
+
 def edge_messages_forward(A, Bm, b1, W, bW, csr: CSRGraph, towers: int, edge_term=None, pitch=None,
                           store_activations: bool = False):
-    """Messages ``[E, T*P]`` in CSR slot order, pad columns zero (and the activations ``[L-1, E, T*F_t]`` when asked)."""
+    """Messages ``[E, T*P]`` in CSR slot order, pad columns zero (and the activations ``[L-1, E, T*F_t]`` when asked), in
+    A's dtype (float32 or bfloat16)."""
     L, T, Ft, P = _check_messages(A, Bm, b1, W, bW, csr, towers, edge_term, pitch)
     A, Bm, b1 = (t.contiguous() for t in (A, Bm, b1))
     W, bW = (W.contiguous(), bW.contiguous()) if L > 1 else (None, None)
     C = None if edge_term is None else edge_term.contiguous()
-    E, dev = csr.n_edges, A.device
-    M = torch.empty((E, T * P), dtype=torch.float32, device=dev)
-    act = torch.empty((L - 1, E, T * Ft), dtype=torch.float32, device=dev) if store_activations and L > 1 else None
+    E, dev, dt = csr.n_edges, A.device, A.dtype
+    M = torch.empty((E, T * P), dtype=dt, device=dev)
+    act = torch.empty((L - 1, E, T * Ft), dtype=dt, device=dev) if store_activations and L > 1 else None
     with torch.cuda.device(dev):
-        _lib.check(_lib.lib().pna_edge_msg_fwd(
+        _lib.check(getattr(_lib.lib(), _KERNEL[dt][0])(
             _ptr(csr.rowptr), _ptr(csr.col) if E else None, csr.n_nodes, E, _ptr(A), _ptr(Bm), _ptr(b1), _ptr(C), _ptr(W),
             _ptr(bW), L, T, Ft, P, _ptr(M), _ptr(act), torch.cuda.current_stream(dev).cuda_stream))
     return M, act
 
 
 def edge_messages_backward(grad_M, pitch: int, act, W, n_layers: int, towers: int, width: int):
-    """``[L-1, E, T*F_t]``: G_1 .. G_(L-1) from ``grad_M [E, T*pitch]`` (L >= 2)."""
-    grad_M, W = grad_M.contiguous().float(), W.contiguous()
+    """``[L-1, E, T*F_t]`` fp32: G_1 .. G_(L-1) from ``grad_M [E, T*pitch]`` (L >= 2), read in the activations' dtype."""
+    grad_M, W = grad_M.contiguous().to(act.dtype), W.contiguous()
     E, dev = grad_M.size(0), grad_M.device
     G = torch.empty((n_layers - 1, E, towers * width), dtype=torch.float32, device=dev)
     with torch.cuda.device(dev):
-        _lib.check(_lib.lib().pna_edge_msg_bwd(_ptr(grad_M), pitch, _ptr(act), _ptr(W), E, n_layers, towers, width, _ptr(G),
-                                               torch.cuda.current_stream(dev).cuda_stream))
+        _lib.check(getattr(_lib.lib(), _KERNEL[act.dtype][1])(_ptr(grad_M), pitch, _ptr(act), _ptr(W), E, n_layers, towers,
+                                                              width, _ptr(G), torch.cuda.current_stream(dev).cuda_stream))
     return G
 
 
@@ -183,6 +202,7 @@ class _EdgeMessages(torch.autograd.Function):
         M, act = edge_messages_forward(A, Bm, b1, W, bW, csr, towers, edge_term, pitch, store_activations=True)
         ctx.save_for_backward(W, act)
         ctx.meta = (csr, towers, Bm.size(0), A.size(1) // towers, M.size(1) // towers)
+        ctx.dtypes = (A.dtype, Bm.dtype, None if edge_term is None else edge_term.dtype)
         return M
 
     @staticmethod
@@ -202,11 +222,14 @@ class _EdgeMessages(torch.autograd.Function):
             # G_k[:, t].  At E = 1.2 M a batched product over the towers instead took the PyG training step of
             # tools/edge_msg_bench.py to 65 ms, against 27 ms (two runs, H100 80GB HBM3, 700 W)
             cols = lambda x, t: x.reshape(E, T, Ft)[:, t]
-            dW = torch.stack([torch.stack([cols(grads[k - 1], t).t() @ cols(act[k - 2], t) for t in range(T)])
+            # (bf16 activations are widened one tower slice at a time: the weight gradients are fp32 GEMMs)
+            dW = torch.stack([torch.stack([cols(grads[k - 1], t).t() @ cols(act[k - 2], t).float() for t in range(T)])
                               for k in range(2, L + 1)])
             dbW = torch.stack([grads[k - 1].reshape(E, T, Ft).sum(0) for k in range(2, L + 1)])
         dA, dBm, db1 = _first_layer_grads(ctx, grads[0], csr, n_src)
         dC = grads[0] if ctx.needs_input_grad[5] else None
+        dt_a, dt_b, dt_c = ctx.dtypes        # each input's gradient in its own dtype (fp32 sums, rounded once)
+        dA, dBm, dC = (None if g is None else g.to(d) for g, d in ((dA, dt_a), (dBm, dt_b), (dC, dt_c)))
         return dA, dBm, db1, dW, dbW, dC, None, None, None
 
 

@@ -17,6 +17,11 @@ Backward: the input gradient runs on the tensor cores (``pna_linear_bwd_data``, 
 never forms the scaled copies).  The weight gradient stays a library fp32 GEMM (``library_grad_weight``): at config 2 on
 H100 cuBLAS is faster than the tensor-core ``pna_linear_bwd_weight`` (DESIGN section 5), which ``linear_bwd_tf32x3``
 still exposes.
+
+Every wrapper of a C entry point checks its operands' dtypes before it allocates or launches anything (``_fp32``): the C
+side takes ``const float*`` and cannot tell a bf16 buffer from an fp32 one.  The one bf16 operand taken is the compact
+tower aggregate (``pna_linear_towers_scaled_fwd_bf16``, the tower layers under bf16 autocast): its output, the data
+gradient and the weight gradient stay fp32, and the data gradient is returned in bf16, the aggregate's dtype.
 """
 from __future__ import annotations
 
@@ -26,7 +31,7 @@ from typing import Optional
 
 import torch
 
-from . import _lib
+from . import _lib, aggregate
 
 _OUT_OK = (64, 128, 256)
 
@@ -39,8 +44,16 @@ def kernel_applies(a: torch.Tensor, weight: torch.Tensor) -> bool:
             and a.data_ptr() % 16 == 0)
 
 
+def _fp32(who: str, **operands) -> None:
+    """TypeError unless every given operand is float32 (None: absent)."""
+    for name, t in operands.items():
+        if t is not None and t.dtype != torch.float32:
+            raise TypeError(f"{who}: {name} is {t.dtype}; the kernel takes float32")
+
+
 def linear_tf32x3(a: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor]) -> torch.Tensor:
     """y = a @ weight.T + bias through the C ABI (no autograd)."""
+    _fp32("linear_tf32x3", a=a, weight=weight, bias=bias)
     n, k = a.shape
     o = weight.size(0)
     dev = a.device
@@ -61,6 +74,7 @@ def linear_bwd_tf32x3(gy: torch.Tensor, a: torch.Tensor, row_scale: Optional[tor
     autograd); a gradient that is not needed is not computed and comes back as None."""
     if not (need_a or need_w):
         return None, None
+    _fp32("linear_bwd_tf32x3", gy=gy, a=a, row_scale=row_scale, weight=weight)
     n, ka = a.shape
     o, k = weight.shape
     s = 1 if row_scale is None else row_scale.size(1)
@@ -141,6 +155,7 @@ def scaled_kernel_applies(a: torch.Tensor, weight: torch.Tensor, n_scalers: int)
 def linear_scaled_tf32x3(a: torch.Tensor, row_scale: torch.Tensor, weight: torch.Tensor,
                          bias: Optional[torch.Tensor]) -> torch.Tensor:
     """y = cat_s(row_scale[:, s, None] * a) @ weight.T + bias through the C ABI (no autograd)."""
+    _fp32("linear_scaled_tf32x3", a=a, row_scale=row_scale, weight=weight, bias=bias)
     n, ka = a.shape
     o, k = weight.shape
     s = row_scale.size(1)
@@ -191,8 +206,10 @@ TOWER_OUT_MAX = 64
 def towers_path_ok(x: torch.Tensor, n_towers: int, n_feat: int, n_out: int, n_scalers: int) -> bool:
     """Shape-level decision the tower layers take BEFORE aggregating: would a fresh fp32 [N, T * (1 + A) * n_feat] compact
     aggregate on x's device, with [T, n_out, (1 + S * A) * n_feat] first post Linears, go through
-    pna_linear_towers_scaled_fwd?  (The layers check the weights' dtype themselves.)"""
-    return (n_scalers > 1 and x.is_cuda and x.dtype == torch.float32 and x.size(0) > 0 and 1 <= n_towers <= TOWERS_MAX
+    pna_linear_towers_scaled_fwd?  (The layers check the weights' dtype themselves.)  Inside autocast the aggregate has the
+    boundary dtype whatever x's (fp32, or bf16 for pna_linear_towers_scaled_fwd_bf16), so x's dtype is not asked."""
+    dtype_ok = aggregate.boundary_dtype() is not None or x.dtype == torch.float32
+    return (n_scalers > 1 and x.is_cuda and dtype_ok and x.size(0) > 0 and 1 <= n_towers <= TOWERS_MAX
             and 1 <= n_out <= TOWER_OUT_MAX and n_towers * n_out <= 256 and n_feat % 4 == 0
             and os.environ.get("PNA_B200_TENSOR_LINEAR", "1") != "0" and os.environ.get("PNA_B200_COMPACT_POST", "1") != "0")
 
@@ -225,7 +242,10 @@ def _tower_dims(a: torch.Tensor, row_scale: torch.Tensor, weight: torch.Tensor):
 def linear_towers_scaled_tf32x3(a: torch.Tensor, row_scale: torch.Tensor, weight: torch.Tensor,
                                 bias: Optional[torch.Tensor]) -> torch.Tensor:
     """y[:, t*O_t:(t+1)*O_t] = [self_t | cat_s(row_scale[:, s, None] * agg_t)] @ weight[t].T + bias[t] through the C ABI
-    (no autograd); a's tower block t is [self_t | agg_t]."""
+    (no autograd); a's tower block t is [self_t | agg_t].  a may be bf16 (pna_linear_towers_scaled_fwd_bf16: y is then
+    what the fp32 call gives on a.float(), bit for bit); y is fp32 either way."""
+    _fp32("linear_towers_scaled_tf32x3", a=None if a.dtype == torch.bfloat16 else a, row_scale=row_scale, weight=weight,
+          bias=bias)
     t, o, fp, n_aggr = _tower_dims(a, row_scale, weight)
     a = a.contiguous()
     n = a.size(0)
@@ -233,16 +253,18 @@ def linear_towers_scaled_tf32x3(a: torch.Tensor, row_scale: torch.Tensor, weight
     w = weight.detach().contiguous()
     b = None if bias is None else bias.detach().contiguous()
     y = torch.empty((n, t * o), dtype=torch.float32, device=dev)
+    entry = "pna_linear_towers_scaled_fwd_bf16" if a.dtype == torch.bfloat16 else "pna_linear_towers_scaled_fwd"
     with torch.cuda.device(dev):
-        _lib.check(_lib.lib().pna_linear_towers_scaled_fwd(a.data_ptr(), a.stride(0), row_scale.data_ptr(), row_scale.size(1),
-                                                           w.data_ptr(), None if b is None else b.data_ptr(), y.data_ptr(), y.stride(0),
-                                                           n, t, fp, n_aggr, o, torch.cuda.current_stream(dev).cuda_stream))
+        _lib.check(getattr(_lib.lib(), entry)(a.data_ptr(), a.stride(0), row_scale.data_ptr(), row_scale.size(1), w.data_ptr(),
+                                              None if b is None else b.data_ptr(), y.data_ptr(), y.stride(0), n, t, fp, n_aggr, o,
+                                              torch.cuda.current_stream(dev).cuda_stream))
     return y
 
 
 def linear_towers_bwd_data(gy: torch.Tensor, row_scale: torch.Tensor, weight: torch.Tensor, a_shape) -> torch.Tensor:
     """grad a of ``linear_towers_scaled_tf32x3`` (no autograd): self columns sum_o gy W_self, aggregate columns
-    sum_s fl(c_s gy) W_s, the scaled copies of gy formed in the kernel's loaders."""
+    sum_s fl(c_s gy) W_s, the scaled copies of gy formed in the kernel's loaders.  fp32 result."""
+    _fp32("linear_towers_bwd_data", gy=gy, row_scale=row_scale, weight=weight)
     t, o, fp, n_aggr = _tower_dims(torch.empty(a_shape, device="meta"), row_scale, weight)
     gy = gy.contiguous()
     n = a_shape[0]
@@ -258,12 +280,13 @@ def linear_towers_bwd_data(gy: torch.Tensor, row_scale: torch.Tensor, weight: to
 
 def library_grad_weight_towers(gy: torch.Tensor, a: torch.Tensor, row_scale: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
     """grad weight of ``linear_towers_scaled_tf32x3``: library fp32 GEMMs, one per tower for the self block and one per
-    tower and scaler for the aggregates, each ``fl(c_s * agg_t)`` a temporary of one tower's aggregate block."""
+    tower and scaler for the aggregates, each ``fl(c_s * agg_t)`` a temporary of one tower's aggregate block.  A bf16 a is
+    widened one tower block at a time, never as a whole."""
     t, o, fp, n_aggr = _tower_dims(a, row_scale, weight)
     af, per = n_aggr * fp, (1 + n_aggr) * fp
     gw = torch.empty_like(weight)
     for k in range(t):
-        gy_t, a_t = gy[:, k * o:(k + 1) * o], a[:, k * per:(k + 1) * per]
+        gy_t, a_t = gy[:, k * o:(k + 1) * o], a[:, k * per:(k + 1) * per].float()
         torch.mm(gy_t.t(), a_t[:, :fp], out=gw[k, :, :fp])
         for s in range(row_scale.size(1)):
             torch.mm(gy_t.t(), a_t[:, fp:] * row_scale[:, s:s + 1], out=gw[k, :, fp + s * af:fp + (s + 1) * af])
@@ -271,7 +294,8 @@ def library_grad_weight_towers(gy: torch.Tensor, a: torch.Tensor, row_scale: tor
 
 
 class _LinearTowersScaled3xTF32(torch.autograd.Function):
-    """Saves the compact aggregate, not the scaled copies.  The scale factors are constants of the graph."""
+    """Saves the compact aggregate (bf16 under bf16 autocast: half the bytes), not the scaled copies.  The scale factors are
+    constants of the graph.  The data gradient is returned in a's dtype."""
 
     @staticmethod
     def forward(ctx, a, row_scale, weight, bias):
@@ -282,7 +306,7 @@ class _LinearTowersScaled3xTF32(torch.autograd.Function):
     @staticmethod
     def backward(ctx, gy):
         a, row_scale, weight = ctx.saved_tensors
-        ga = linear_towers_bwd_data(gy, row_scale, weight, a.shape) if ctx.needs_input_grad[0] else None
+        ga = linear_towers_bwd_data(gy, row_scale, weight, a.shape).to(a.dtype) if ctx.needs_input_grad[0] else None
         gw = library_grad_weight_towers(gy, a, row_scale, weight) if ctx.needs_input_grad[2] else None
         gb = gy.sum(0).view(weight.size(0), weight.size(1)) if (ctx.has_bias and ctx.needs_input_grad[3]) else None
         return ga, None, gw, gb

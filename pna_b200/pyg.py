@@ -13,8 +13,8 @@ import torch
 from torch import Tensor
 from torch.nn import Linear, Module, ModuleList, ReLU, Sequential
 
-from . import _lib, padding as pad
-from .aggregate import avg_deg_from_histogram, pna_aggregate, row_scales
+from . import _lib, aggregate, padding as pad
+from .aggregate import at_boundary, avg_deg_from_histogram, pna_aggregate, row_scales
 from . import edge_mlp
 from .edge_mlp import edge_messages
 from .linear import compact_path_ok, linear_tf32x3, post_linear, post_linear_scaled, post_linear_towers_scaled, towers_compact_pays, towers_path_ok
@@ -171,6 +171,11 @@ class PNAConv(Module):
     (the towers' ``pre_nns`` on gathered rows) only for inputs the kernel does not take: dtypes other than float32, and
     ``pre_layers > 1`` with a tower width ``F_in`` above 64 -- and for training steps on graphs below
     ``edge_mlp.FUSED_TRAINING_MIN_EDGES`` edges, where the torch path measured faster (launch overhead).
+
+    Under ``torch.autocast("cuda")`` the operands of the kernels take ``aggregate.boundary_dtype()`` (DESIGN section 2):
+    with bf16 the GEMM products U / V, A / Bm / C stay bf16 and run the bf16 aggregation, messages and compact tower
+    post-linear, whatever x's dtype; with fp16 they are upcast to fp32 and run the fp32 kernels.  The tower width is padded
+    for that dtype.  The weights stay fp32 throughout.
     """
 
     def __init__(self, in_channels: int, out_channels: int, aggregators: List[str], scalers: List[str], deg: Tensor,
@@ -261,8 +266,10 @@ class PNAConv(Module):
 
     def _fused_messages_ok(self, x: Tensor, edge_attr: Optional[Tensor], n_edges: int) -> bool:
         """The inputs pna_edge_msg_fwd takes: float32 on the GPU, and a tower width of at most 64 with pre_layers > 1;
-        with autograd, graphs of at least edge_mlp.FUSED_TRAINING_MIN_EDGES edges (where the kernel path is faster)."""
-        return (edge_mlp.fused_step_pays(n_edges) and x.is_cuda and x.dtype == torch.float32 and self.pre_nns[0][0].weight.dtype == torch.float32
+        with autograd, graphs of at least edge_mlp.FUSED_TRAINING_MIN_EDGES edges (where the kernel path is faster).
+        Inside autocast the GEMMs make the operands, in the boundary dtype: x's own dtype is not asked, the weights' is."""
+        x_ok = x.dtype == torch.float32 or aggregate.boundary_dtype() is not None
+        return (edge_mlp.fused_step_pays(n_edges) and x.is_cuda and x_ok and self.pre_nns[0][0].weight.dtype == torch.float32
                 and (edge_attr is None) == (self.edge_dim is None)
                 and (self.pre_layers == 1 or self.F_in <= _lib.EDGE_MLP_MAX_WIDTH))
 
@@ -273,8 +280,8 @@ class PNAConv(Module):
         Wi, Wj, b1, We, W, bW = self._message_weights()
         C = None
         if edge_attr is not None:
-            C = self.edge_encoder(edge_attr).index_select(0, csr.perm.long()) @ We.t()
-        return edge_messages(x @ Wi.t(), x @ Wj.t(), b1, W, bW, csr, self.towers, edge_term=C, pitch=Fp)
+            C = at_boundary(self.edge_encoder(edge_attr).index_select(0, csr.perm.long()) @ We.t())
+        return edge_messages(at_boundary(x @ Wi.t()), at_boundary(x @ Wj.t()), b1, W, bW, csr, self.towers, edge_term=C, pitch=Fp)
 
     def _message_weights(self):
         """The pre_nns weights packed as the kernel takes them, cached per parameter version like ``_prepared``."""
@@ -393,7 +400,7 @@ class PNAConv(Module):
                 deg: Optional[Tensor] = None, csr: Optional[CSRGraph] = None) -> Tensor:
         csr = _resolve_csr(x, edge_index, csr)
         T, Fi = self.towers, self.F_in
-        Fp = pad.padded_width(Fi, x.dtype)
+        Fp = pad.padded_width(Fi, aggregate.boundary_dtype() or x.dtype)      # the kernels' dtype: bf16 pads to 8 columns
         # self features at the (possibly padded) tower width
         if Fp == Fi:
             x_self = x
@@ -407,13 +414,13 @@ class PNAConv(Module):
         compact = self._compact(x, Fp)
         scalers = ["identity"] if compact else self.scalers
         if edge_attr is None and self.pre_layers == 1 and self.edge_dim is None:
-            U, V = self._affine_terms(x, Fp)
+            U, V = (at_boundary(t) for t in self._affine_terms(x, Fp))
             out = pna_aggregate(V, csr, self.aggregators, scalers, self.avg_deg, row_bias=U, **common)
         else:
             if self._fused_messages_ok(x, edge_attr, csr.n_edges):
                 msgs = self._fused_messages(x, csr, edge_attr, Fp)
             else:
-                msgs = pad.pad_blocks(self._messages_in_slot_order(x, csr, edge_attr), T, Fi, Fp)
+                msgs = at_boundary(pad.pad_blocks(self._messages_in_slot_order(x, csr, edge_attr), T, Fi, Fp))
             out = pna_aggregate(msgs, csr, self.aggregators, scalers, self.avg_deg, messages_in_csr_order=True,
                                 **common)
         w_post, b_post = self._prepared(Fp)[2:]

@@ -5,6 +5,8 @@ The reference nets finish with ``dgl.sum_nodes / mean_nodes / max_nodes(g, 'h')`
 a segmented reduction of node rows by graph id.  That is the aggregation path with "destination" = graph and
 "source" = node, so it runs on ``pna_aggregate_fwd`` / ``pna_aggregate_bwd`` unchanged (graphs larger than the split
 threshold become split rows); no separate kernel, no atomics, deterministic.  Empty graphs give zero rows.
+Inside ``torch.autocast("cuda")`` an fp16 input (an autocast Linear's output) is upcast to fp32 at the kernel boundary;
+fp32 and bf16 inputs are reduced in their own dtype (DESIGN section 2).
 """
 from __future__ import annotations
 
@@ -13,7 +15,7 @@ from typing import Optional
 
 import torch
 
-from .aggregate import pna_aggregate
+from .aggregate import at_boundary, pna_aggregate
 from .csr import CSRGraph, build_csr, tensor_version
 
 _UNIT = {"log": 1.0, "lin": 1.0}        # identity scaler only: the averages are never read
@@ -44,7 +46,7 @@ def segment_reduce(x: torch.Tensor, batch: torch.Tensor, n_graphs: Optional[int]
         raise ValueError("x must be [N, F] and batch [N]")
     if n_graphs is None:
         n_graphs = int(batch.max()) + 1 if batch.numel() else 0
-    return pna_aggregate(x, batch_csr(batch, n_graphs), [reduce], ["identity"], _UNIT)
+    return pna_aggregate(at_boundary(x), batch_csr(batch, n_graphs), [reduce], ["identity"], _UNIT)
 
 
 def global_add_pool(x: torch.Tensor, batch: torch.Tensor, size: Optional[int] = None) -> torch.Tensor:
