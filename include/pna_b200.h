@@ -39,7 +39,9 @@ enum pna_status {
   PNA_ERR_UNSUPPORTED = -2, /* dtype / size outside what the kernels take (e.g. E >= 2^31) */
   PNA_ERR_CUDA = -3,        /* a CUDA runtime call failed; message carries cudaGetErrorString */
   PNA_ERR_INDEX = -4,       /* an edge endpoint outside [0, n_nodes) was found while building the CSR */
-  PNA_ERR_WORKSPACE = -5    /* caller-provided workspace / capacity too small */
+  PNA_ERR_WORKSPACE = -5,   /* caller-provided workspace / capacity too small */
+  PNA_ERR_CAPTURING = -6    /* the stream is capturing a CUDA graph and the call would synchronise or read back; nothing
+                               was enqueued (pna_csr_build, pna_csr_light_view: build per-graph state before the capture) */
 };
 
 enum pna_dtype { PNA_F32 = 0, PNA_BF16 = 1 };
@@ -151,14 +153,16 @@ int pna_csr_workspace_bytes(int64_t n_nodes, int64_t n_edges, size_t* bytes);
 
 /* src[e] -> dst[e], e in [0, n_edges): int64 device arrays (edge_index[0], edge_index[1] of PyG;
  * g.edges() of DGL).  Synchronises the stream once at the end to return the host-side counts and to report
- * out-of-range endpoints (PNA_ERR_INDEX).  Call once per graph, not per layer. */
+ * out-of-range endpoints (PNA_ERR_INDEX).  Call once per graph, not per layer.  On a stream that is capturing a CUDA graph
+ * it returns PNA_ERR_CAPTURING before it enqueues anything. */
 int pna_csr_build(const int64_t* src, const int64_t* dst, pna_csr_t* csr, void* workspace, size_t workspace_bytes,
                   pna_stream_t stream);
 
 /* Light view restricted to the rows with row_mask[r] != 0 (NULL = all rows below the split threshold); rows outside
  * the mask get light_deg = -1 and no slots, so the streaming kernel skips them without a row list.  Used to run the
  * rows whose sources are all local while the halo all-to-all is in flight, then the rest.  workspace: at least
- * pna_csr_light_view_workspace_bytes(n_nodes) bytes of device scratch. */
+ * pna_csr_light_view_workspace_bytes(n_nodes) bytes of device scratch.  Per-graph state like the CSR: on a stream that is
+ * capturing a CUDA graph it returns PNA_ERR_CAPTURING before it enqueues anything. */
 int pna_csr_light_view(const int32_t* rowptr, const int32_t* col, int64_t n_nodes, int32_t split_threshold, const uint8_t* row_mask,
                        int32_t n_part, int32_t* light_rowptr, int32_t* light_deg, int32_t* light_col, int32_t* part,
                        void* workspace, size_t workspace_bytes, pna_stream_t stream);

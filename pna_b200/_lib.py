@@ -31,6 +31,7 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-
 # status codes / enums of include/pna_b200.h
 ABI_VERSION = 8
 PNA_OK = 0
+PNA_ERR_CAPTURING = -6     # pna_csr_build / pna_csr_light_view on a stream that is capturing a CUDA graph
 PNA_F32, PNA_BF16 = 0, 1
 AGGR_CODES = {"sum": 0, "mean": 1, "min": 2, "max": 3, "var": 4, "std": 5, "_skip": 15}
 # the central moments of the dense registry (PNA_AGGR_MOMENT3..5): a separate table, merged where the aggregation packs its

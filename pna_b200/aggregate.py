@@ -12,7 +12,7 @@ from typing import Mapping, Optional, Sequence, Union
 
 import torch
 
-from . import _lib
+from . import _lib, capture
 from .csr import CSRGraph
 
 _DTYPES = {torch.float32: _lib.PNA_F32, torch.bfloat16: _lib.PNA_BF16}
@@ -200,6 +200,7 @@ def aggregate_forward(gathered: torch.Tensor, csr: CSRGraph, aggregators: Names,
         if ptr_table.dtype != torch.int64 or ptr_table.device != dev:
             raise ValueError("peer pointer table must be an int64 tensor on the same device")
         d.peer_gathered, d.peer_shift = ptr_table.data_ptr(), int(shift)
+    capture.pin(csr, view, scaler_degree, degree_col)
     with torch.cuda.device(dev):
         _lib.check(_lib.lib().pna_aggregate_fwd(C.byref(d), torch.cuda.current_stream(dev).cuda_stream))
     return out
@@ -213,6 +214,7 @@ def row_scales(csr: CSRGraph, scalers: Names, avg_deg: Mapping[str, float]) -> t
     cache = csr.__dict__.setdefault("_row_scale_cache", {})
     hit = cache.get(key)
     if hit is not None:
+        capture.pin(csr, hit)
         return hit
     dev = csr.device
     out = torch.empty((csr.n_nodes, n_scal), dtype=torch.float32, device=dev)
@@ -222,6 +224,7 @@ def row_scales(csr: CSRGraph, scalers: Names, avg_deg: Mapping[str, float]) -> t
     if len(cache) > 8:
         cache.clear()
     cache[key] = out
+    capture.pin(csr, out)
     return out
 
 
@@ -236,6 +239,7 @@ def aggregate_backward(grad_out: torch.Tensor, gathered: torch.Tensor, csr: CSRG
     gathered = _rows2d(gathered, "gathered")
     F = int(gathered.size(1))
     N = csr.n_nodes
+    capture.pin(csr, scaler_degree, degree_col)
     n_aggr, aggr_codes = _lib.pack_codes(aggregators, _lib.ALL_AGGR_CODES, "aggregator")
     n_scal, scal_codes = _lib.pack_codes(scalers, _lib.SCALER_CODES, "scaler")
     grad_out = _rows2d(grad_out.to(gathered.dtype), "grad_out")

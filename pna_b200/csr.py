@@ -14,7 +14,7 @@ from typing import Optional
 
 import torch
 
-from . import _lib
+from . import _lib, capture
 
 
 @dataclass
@@ -111,6 +111,7 @@ class CSRGraph:
         key = ("T", int(n_src))
         t = self._partials.get(key)
         if t is None:
+            capture.guard("the transposed CSR of this graph (the coefficient backward)")
             t = build_csr(self.dst_of_slot, self.col.long(), int(n_src), n_src=self.n_nodes)
             self._partials[key] = t
         return t
@@ -122,12 +123,14 @@ class CSRGraph:
         key = ("S", int(n_src))
         t = self._partials.get(key)
         if t is None:
+            capture.guard("the slot-transposed CSR of this graph (the deterministic and edge-message backwards)")
             t = build_csr(torch.arange(self.n_edges, device=self.device), self.col.long(), int(n_src), n_src=self.n_edges)
             self._partials[key] = t
         return t
 
     def masked_view(self, row_mask: torch.Tensor) -> LightView:
         """Light view of the rows with ``row_mask != 0`` only (uint8/bool [N]); other rows are skipped by the kernel."""
+        capture.guard("CSRGraph.masked_view (a light view is per-graph state)", "build the view before the capture")
         N, dev = self.n_nodes, self.device
         mask = row_mask.to(device=dev, dtype=torch.uint8).contiguous()
         if mask.numel() != N:
@@ -163,7 +166,11 @@ def build_csr(src: torch.Tensor, dst: torch.Tensor, n_nodes: int, split_threshol
     """Build the CSR on the GPU through the C ABI.  ``src[e] -> dst[e]``; int64 CUDA tensors.
 
     ``n_src`` (default ``n_nodes``): number of source rows when they differ from the destination rows -- the
-    destination-partitioned multi-GPU path gathers from ``[local rows ; halo rows]``."""
+    destination-partitioned multi-GPU path gathers from ``[local rows ; halo rows]``.
+
+    Reads its counters back (one stream synchronisation), so inside a CUDA graph capture it raises
+    ``capture.CaptureError`` instead (the graph's first eager step builds the CSR)."""
+    capture.guard("build_csr (the CSR of a graph not seen before)")
     if not src.is_cuda or not dst.is_cuda:
         raise ValueError("pna_b200.build_csr needs CUDA tensors (there is no CPU path)")
     if src.dtype != torch.int64 or dst.dtype != torch.int64:
@@ -237,6 +244,7 @@ def csr_from_edge_index(edge_index: torch.Tensor, n_nodes: int, cache: bool = Tr
         hit = _CACHE.get(key)
         if hit is not None:
             _CACHE.move_to_end(key)
+            capture.pin(hit[1])
             return hit[1]
     g = build_csr(edge_index[0], edge_index[1], n_nodes)
     if cache:

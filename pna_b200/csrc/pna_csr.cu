@@ -215,6 +215,16 @@ static int light_view(const int* rowptr, const int* col, long long N, long long 
   return PNA_OK;
 }
 
+// Building per-graph state reads counters back (pna_csr_build) and belongs before a CUDA graph capture, not in it: on a
+// capturing stream both builders return PNA_ERR_CAPTURING before anything is enqueued, so the capture stays intact.
+static int refuse_capture(cudaStream_t st, const char* who) {
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  PNA_CUDA_TRY(cudaStreamIsCapturing(st, &cs));
+  PNA_REQUIRE(cs == cudaStreamCaptureStatusNone, PNA_ERR_CAPTURING,
+              "%s: the stream is capturing a CUDA graph; build the graph's CSR and views before the capture", who);
+  return PNA_OK;
+}
+
 }  // namespace pna
 
 using namespace pna;
@@ -230,6 +240,8 @@ extern "C" int pna_csr_light_view(const int32_t* rowptr, const int32_t* col, int
   const size_t scan_in_bytes = align_up((size_t)(n_nodes + 1) * sizeof(int), 256);
   const size_t need = scan_in_bytes + align_up(scan_bytes, 256);
   PNA_REQUIRE(workspace != nullptr && workspace_bytes >= need, PNA_ERR_WORKSPACE, "pna_csr_light_view: workspace %zu bytes < required %zu", workspace_bytes, need);
+  const int rc = refuse_capture(static_cast<cudaStream_t>(stream), "pna_csr_light_view");
+  if (rc != PNA_OK) return rc;
   char* ws = static_cast<char*>(workspace);
   ChunkRows none = {nullptr, nullptr, nullptr, 1};
   return light_view(rowptr, col, n_nodes, n_nodes, split_threshold, row_mask, none, n_part, light_rowptr, light_deg, light_col, part,
@@ -281,6 +293,8 @@ extern "C" int pna_csr_build(const int64_t* src, const int64_t* dst, pna_csr_t* 
   PNA_REQUIRE(workspace != nullptr && workspace_bytes >= L.total, PNA_ERR_WORKSPACE,
               "pna_csr_build: workspace %zu bytes < required %zu", workspace_bytes, L.total);
   PNA_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255u) == 0, PNA_ERR_BAD_ARG, "pna_csr_build: workspace must be 256-byte aligned");
+  rc = refuse_capture(static_cast<cudaStream_t>(stream), "pna_csr_build");     // after the argument checks, before any work
+  if (rc != PNA_OK) return rc;
 
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   char* ws = static_cast<char*>(workspace);

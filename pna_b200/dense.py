@@ -47,7 +47,7 @@ import torch.nn as nn
 from .aggregate import aggregate_forward, at_boundary, pna_aggregate
 from .csr import build_csr, tensor_version
 from .edge_mlp import edge_mlp
-from . import _lib
+from . import _lib, capture
 from .nn_blocks import FCLayer, MLP
 
 _SELF_FIRST = ("mean", "std", "sum", "var", "moment3", "moment4", "moment5", "softmax", "softmin", "normalised_mean")
@@ -59,6 +59,7 @@ class DenseGraphs:
     """Block-diagonal CSRs of a dense batch: one for adj (row i gathers j) and one for adj^T."""
 
     def __init__(self, adj: torch.Tensor, self_loop: bool = False):
+        capture.guard("DenseGraphs (the CSRs of a dense batch not seen before: adj.nonzero)")
         B, N, _ = adj.shape
         a = adj
         if self_loop:
@@ -95,6 +96,7 @@ def dense_graphs(adj: torch.Tensor, self_loop: bool) -> DenseGraphs:
             _CACHE.clear()
         hit = (adj, DenseGraphs(adj, self_loop))
         _CACHE[key] = hit
+    capture.pin(hit[1])
     return hit[1]
 
 
@@ -153,15 +155,21 @@ class PNALayer(nn.Module):
 
     def _columns(self, width, a2, device):
         """bool [width]: output columns of the list positions of ``a2`` that are not "_skip" (per tower: self block, then
-        S x A blocks of F_t) -- those of the max/min call, or of ``identity``."""
-        T, Ft = len(self.towers), self.input_tower
-        A, S = len(self.aggregators), len(self.scalers)
-        m = torch.zeros(T, 1 + S * A, Ft, dtype=torch.bool)
-        for s_ in range(S):
-            for a_, name in enumerate(a2):
-                if name != "_skip":
-                    m[:, 1 + s_ * A + a_, :] = True
-        return m.reshape(-1)[:width].to(device)
+        S x A blocks of F_t) -- those of the max/min call, or of ``identity``.  Made once per layer and device: a copy
+        from host memory cannot run inside a CUDA graph capture."""
+        key = (width, tuple(a2), str(device))
+        masks = self.__dict__.setdefault("_column_masks", {})
+        if key not in masks:
+            capture.guard("dense PNALayer's column mask (a host-to-device copy)", "run one eager step of this layer first")
+            T, Ft = len(self.towers), self.input_tower
+            A, S = len(self.aggregators), len(self.scalers)
+            m = torch.zeros(T, 1 + S * A, Ft, dtype=torch.bool)
+            for s_ in range(S):
+                for a_, name in enumerate(a2):
+                    if name != "_skip":
+                        m[:, 1 + s_ * A + a_, :] = True
+            masks[key] = m.reshape(-1)[:width].to(device)
+        return masks[key]
 
     def forward(self, input, adj):
         B, N, Fin = input.shape

@@ -25,7 +25,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import _lib, aggregate, padding as pad
+from . import _lib, aggregate, capture, padding as pad
 from .aggregate import at_boundary, pna_aggregate, row_scales
 from . import edge_mlp
 from .edge_mlp import edge_messages
@@ -123,12 +123,13 @@ class PNALayer(nn.Module):
         """pretrans(cat[src h, dst h]) = W_s h_src + W_d h_dst + b (pna_layer.py:35-40): V = h W_s^T + b, U = h W_d^T,
         each tower block padded to fp columns with zero weight rows.  Both come out of ONE GEMM against the packed weight
         [W_d ; W_s] (block-diagonal per tower with divide_input), which is rebuilt only when a parameter changed (without
-        autograd; with autograd it is part of the graph and rebuilt every call)."""
+        autograd; with autograd it is part of the graph and rebuilt every call; inside a CUDA graph capture it is rebuilt and
+        not cached, so that a replay follows the weights)."""
         it = self.input_tower
         lins = [tw.pretrans.fully_connected[0].linear for tw in self.towers]
         params = [p_ for l in lins for p_ in (l.weight, l.bias)]
         key = (fp, tuple(tensor_version(p_) for p_ in params), tuple(p_.data_ptr() for p_ in params))
-        cache = not (torch.is_grad_enabled() and any(p_.requires_grad for p_ in params))
+        cache = not (torch.is_grad_enabled() and any(p_.requires_grad for p_ in params)) and not capture.capturing()
         hit = getattr(self, "_uv_pack", None)
         if cache and hit is not None and hit[0] == key:
             w_uv, b_uv = hit[1]
@@ -176,7 +177,7 @@ class PNALayer(nn.Module):
         fcs = [tw.pretrans.fully_connected for tw in self.towers]
         params = [p_ for f in fcs for fc in f for p_ in (fc.linear.weight, fc.linear.bias)]
         key = (tuple(tensor_version(p_) for p_ in params), tuple(p_.data_ptr() for p_ in params))
-        cache = not (torch.is_grad_enabled() and any(p_.requires_grad for p_ in params))
+        cache = not (torch.is_grad_enabled() and any(p_.requires_grad for p_ in params)) and not capture.capturing()
         hit = getattr(self, "_msg_pack", None)
         if cache and hit is not None and hit[0] == key:
             return hit[1]

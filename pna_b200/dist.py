@@ -33,9 +33,14 @@ from typing import List, Optional
 import torch
 import torch.distributed as dist
 
-from . import _lib
+from . import _lib, capture
 from .aggregate import _DTYPES, _names, _rows2d, aggregate_forward, deterministic_slab_width, pna_aggregate
 from .csr import LightView, build_csr
+
+
+def _refuse_capture(plane) -> None:
+    """The planes wait on their peers (barriers with timeouts, collectives, status read-backs): not capturable."""
+    capture.guard(f"{type(plane).__name__} (a multi-GPU plane)", "the multi-GPU planes run eagerly only")
 
 
 # ---- partitioning ------------------------------------------------------------------------------------------------
@@ -163,6 +168,7 @@ class _TrainableExchange:
         ``[n_local, width]`` output.  Every rank must make the same sequence of calls (each one exchanges the halo in the
         forward and, if a gradient flows, returns it in the backward).  Gradients of parameters that produced ``x`` are
         this rank's partial sums: all-reduce them across ranks before the optimizer step."""
+        _refuse_capture(self)
         if x.requires_grad and torch.is_grad_enabled() and not self.trainable:
             raise RuntimeError(f"a gradient through the halo exchange needs {type(self).__name__}(..., trainable=True)")
         x_ext = _HaloExchange.apply(x, self)
@@ -218,6 +224,7 @@ class HaloAggregator(_TrainableExchange):
         return self.x_ext[: self.plan.n_local]
 
     def _exchange_into(self, x_ext: torch.Tensor) -> None:
+        _refuse_capture(self)
         p = self.plan
         gather_rows(x_ext[:p.n_local], p.send_idx, self.send_buf)
         self._all_to_all(x_ext[p.n_local:], self.send_buf, output_split_sizes=p.recv_splits,
@@ -242,6 +249,7 @@ class HaloAggregator(_TrainableExchange):
         all-to-all with the split sizes swapped; the halo is grouped by owner, so nothing is packed); returns a fp32 copy of
         ``grad_ext[:n_local]`` plus the gradients every peer returned for copies of this rank's rows
         (``pna_halo_grad_pull``, its pointer table aimed at the peers' segments of the local receive buffer)."""
+        _refuse_capture(self)
         p, gp = self.plan, self.grad_plan
         if not self.trainable:
             raise RuntimeError("the gradient return needs HaloAggregator(..., trainable=True)")
@@ -259,6 +267,7 @@ class HaloAggregator(_TrainableExchange):
         return g
 
     def aggregate(self, aggregators, scalers, avg_deg, out: Optional[torch.Tensor] = None, **kw) -> torch.Tensor:
+        _refuse_capture(self)
         main = torch.cuda.current_stream(self.x_ext.device)
         if not self.overlap:
             self.exchange()
@@ -598,6 +607,7 @@ class PullAggregator(_TrainableExchange):
                                                    self._status.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
 
     def exchange(self) -> None:
+        _refuse_capture(self)
         p = self.plan
         if self.use_barrier:
             self.barrier()
@@ -638,6 +648,7 @@ class PullAggregator(_TrainableExchange):
     def pull_halo_grad(self, grad_ext: torch.Tensor) -> torch.Tensor:
         """Backward, second half: barrier, then a fp32 copy of ``grad_ext[:n_local]`` plus the gradients every peer staged
         for copies of this rank's rows (``pna_halo_grad_pull``); flips to the other gradient buffer."""
+        _refuse_capture(self)
         p, gp = self.plan, self.grad_plan
         if not self.trainable:
             raise RuntimeError("the gradient return needs PullAggregator(..., trainable=True)")
@@ -661,6 +672,7 @@ class PullAggregator(_TrainableExchange):
 
     def check(self) -> None:
         """Host-side check (synchronises): did every barrier see all peers arrive?"""
+        _refuse_capture(self)
         if int(self._status.item()) != 0:
             raise RuntimeError("pna_peer_barrier timed out: a peer rank did not reach the barrier")
 
@@ -777,6 +789,7 @@ class PeerAggregator:
 
     def barrier(self) -> None:
         """All ranks have finished writing their x rows (device-side, on the current stream)."""
+        _refuse_capture(self)
         h = self._keep.get("handle") if isinstance(self._keep, dict) else None
         if h is not None and hasattr(h, "barrier"):
             h.barrier()
@@ -784,6 +797,7 @@ class PeerAggregator:
             dist.barrier(group=self.group, device_ids=[self.x_local.device.index])
 
     def aggregate(self, aggregators, scalers, avg_deg, out: Optional[torch.Tensor] = None, **kw) -> torch.Tensor:
+        _refuse_capture(self)
         return aggregate_forward(self.x_local, self.csr, aggregators, scalers, avg_deg, out=out,
                                  peer=(self.ptr_table, self.shift), **kw)
 
@@ -803,6 +817,7 @@ class PeerAggregator:
 
     def check(self) -> None:
         """Host-side check (synchronises): did every barrier of the trainable path see all peers arrive?"""
+        _refuse_capture(self)
         if self.trainable and int(self._status.item()) != 0:
             raise RuntimeError("pna_peer_barrier timed out: a peer rank did not reach the barrier")
 
@@ -813,6 +828,7 @@ class PeerAggregator:
         """Differentiable aggregation of this rank's rows, gathered over NVLink: x is the rank's ``[n_local, F]``
         features, ``row_bias`` / ``self_feat`` are per destination and stay local; returns the rank's ``[n_local, width]``
         output.  Needs ``trainable=True``; the rules on the call sequence are in the class docstring."""
+        _refuse_capture(self)
         if not self.trainable:
             raise RuntimeError("PeerAggregator.pna_aggregate needs PeerAggregator(..., trainable=True)")
         if tuple(x.shape) != (self.n_local, self.n_feat) or x.dtype != self.dtype:

@@ -24,7 +24,7 @@ from __future__ import annotations
 
 import torch
 
-from . import _lib
+from . import _lib, capture
 from .aggregate import aggregate_forward
 from .csr import CSRGraph
 
@@ -65,6 +65,7 @@ def edge_mlp_forward(A, Bm, b1, W, bW, csr: CSRGraph, towers: int, store_activat
     E, dev = csr.n_edges, A.device
     M = torch.empty((E, T * Ft), dtype=torch.float32, device=dev)
     act = torch.empty((L - 1, E, T * Ft), dtype=torch.float32, device=dev) if store_activations else None
+    capture.pin(csr)
     with torch.cuda.device(dev):
         _lib.check(_lib.lib().pna_edge_mlp_fwd(
             _ptr(csr.rowptr), _ptr(csr.col) if E else None, csr.n_nodes, E, _ptr(A), _ptr(Bm), _ptr(b1), _ptr(W), _ptr(bW),
@@ -178,6 +179,7 @@ def edge_messages_forward(A, Bm, b1, W, bW, csr: CSRGraph, towers: int, edge_ter
     E, dev, dt = csr.n_edges, A.device, A.dtype
     M = torch.empty((E, T * P), dtype=dt, device=dev)
     act = torch.empty((L - 1, E, T * Ft), dtype=dt, device=dev) if store_activations and L > 1 else None
+    capture.pin(csr)
     with torch.cuda.device(dev):
         _lib.check(getattr(_lib.lib(), _KERNEL[dt][0])(
             _ptr(csr.rowptr), _ptr(csr.col) if E else None, csr.n_nodes, E, _ptr(A), _ptr(Bm), _ptr(b1), _ptr(C), _ptr(W),

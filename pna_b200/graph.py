@@ -11,6 +11,7 @@ from typing import Optional
 
 import torch
 
+from . import capture
 from .csr import CSRGraph, build_csr, tensor_version
 
 _ATTR = "_pna_b200_csr"
@@ -71,6 +72,7 @@ def graph_csr(g, device: torch.device) -> CSRGraph:
         stamp += (src.data_ptr(), dst.data_ptr(), tensor_version(src), tensor_version(dst))
     hit = getattr(g, _ATTR, None)
     if hit is not None and hit[0] == stamp and hit[1].device == device:
+        capture.pin(hit[1])
         return hit[1]
     csr = build_csr(src.to(device), dst.to(device), n)
     try:

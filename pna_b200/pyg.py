@@ -13,7 +13,7 @@ import torch
 from torch import Tensor
 from torch.nn import Linear, Module, ModuleList, ReLU, Sequential
 
-from . import _lib, aggregate, padding as pad
+from . import _lib, aggregate, capture, padding as pad
 from .aggregate import at_boundary, avg_deg_from_histogram, pna_aggregate, row_scales
 from . import edge_mlp
 from .edge_mlp import edge_messages
@@ -232,10 +232,11 @@ class PNAConv(Module):
                                       divide_input: tower t only sees its own F_in input columns (block-diagonal);
           w_post [T, F_out, (1+S*A)*Fp], b_post [T, F_out] -- first post Linear of every tower with zero columns at the pad
                                       positions: ONE batched GEMM over all towers (pna.py:132).
-        With autograd enabled the pack is rebuilt every call (it is part of the graph); otherwise it is cached."""
+        With autograd enabled the pack is rebuilt every call (it is part of the graph); otherwise it is cached, except
+        inside a CUDA graph capture, where the packing is captured so that a replay follows the weights."""
         params = [p_ for nn in list(self.pre_nns) + list(self.post_nns) for p_ in nn[0].parameters()]
         key = (Fp, tuple(tensor_version(p_) for p_ in params), tuple(p_.data_ptr() for p_ in params))
-        cache = torch.is_grad_enabled() is False or not any(p_.requires_grad for p_ in params)
+        cache = (torch.is_grad_enabled() is False or not any(p_.requires_grad for p_ in params)) and not capture.capturing()
         if cache and getattr(self, "_prep", None) is not None and self._prep[0] == key:
             return self._prep[1]
         T, Fi = self.towers, self.F_in
@@ -289,7 +290,7 @@ class PNAConv(Module):
         lins = [list(nn)[0::2] for nn in self.pre_nns]           # the Linears of each tower (ReLU between them)
         params = [p_ for l in lins for lin in l for p_ in lin.parameters()]
         key = (tuple(tensor_version(p_) for p_ in params), tuple(p_.data_ptr() for p_ in params))
-        cache = torch.is_grad_enabled() is False or not any(p_.requires_grad for p_ in params)
+        cache = (torch.is_grad_enabled() is False or not any(p_.requires_grad for p_ in params)) and not capture.capturing()
         if cache and getattr(self, "_msg_pack", None) is not None and self._msg_pack[0] == key:
             return self._msg_pack[1]
         W1 = [l[0].weight for l in lins]
@@ -332,10 +333,12 @@ class PNAConv(Module):
           towers   [N, T*W -> K2] x [O2, K2]: BLOCK-DIAGONAL -- output columns t*F_out.. read only tower t's W input
                    columns, so one launch does the first post Linear of every tower (pna.py:132) and its output is already
                    the concatenation torch.cat(outs, dim=1) of pna.py:134;
-          lin      [N, O2] x [O3, O2]:        the final Linear (pna.py:135) on that buffer; pad columns meet zero weights."""
+          lin      [N, O2] x [O3, O2]:        the final Linear (pna.py:135) on that buffer; pad columns meet zero weights.
+        Inside a CUDA graph capture the pack is built every call and not cached (``_prepared``)."""
         params = [p_ for nn in list(self.pre_nns) + list(self.post_nns) for p_ in nn[0].parameters()] + list(self.lin.parameters())
         key = ("tc", Fp, tuple(tensor_version(p_) for p_ in params), tuple(p_.data_ptr() for p_ in params))
-        if getattr(self, "_tc", None) is not None and self._tc[0] == key:
+        cache = not capture.capturing()
+        if cache and getattr(self, "_tc", None) is not None and self._tc[0] == key:
             return self._tc[1]
         up32 = lambda v: (v + 31) // 32 * 32
         pick = lambda v: 64 if v <= 64 else 128 if v <= 128 else 256
@@ -356,7 +359,8 @@ class PNAConv(Module):
         w3 = torch.zeros((O3, O2), dtype=dt, device=dev); w3[: self.out_channels, : T * Fo] = self.lin.weight
         b3 = torch.zeros(O3, dtype=dt, device=dev); b3[: self.out_channels] = self.lin.bias
         pack = dict(K1=K1, w1=w1, b1=b1, K2=K2, w2=w2, b2=b2, w3=w3, b3=b3)
-        self._tc = (key, pack)
+        if cache:
+            self._tc = (key, pack)
         return pack
 
     def _tensor_core_ok(self, x: Tensor, edge_attr, Fp: int) -> bool:
@@ -381,6 +385,7 @@ class PNAConv(Module):
         if buf is None or buf.size(0) != N or buf.size(1) != tc["K2"] or buf.device != x.device:
             buf = torch.zeros((N, tc["K2"]), dtype=torch.float32, device=x.device)
             self._tc_buf = buf
+        capture.pin(buf)           # a later call on another N replaces it
         aggregate_forward(V, csr, self.aggregators, self.scalers, self.avg_deg, towers=T, row_bias=U, self_feat=x_self,
                           self_divided=self.divide_input, out=buf[:, :width] if width < tc["K2"] else buf)
         h = linear_tf32x3(buf, tc["w2"], tc["b2"])                                               # [N, O2] = cat over towers | 0

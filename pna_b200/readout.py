@@ -15,6 +15,7 @@ from typing import Optional
 
 import torch
 
+from . import capture
 from .aggregate import at_boundary, pna_aggregate
 from .csr import CSRGraph, build_csr, tensor_version
 
@@ -28,6 +29,7 @@ def batch_csr(batch: torch.Tensor, n_graphs: int) -> CSRGraph:
     hit = _CACHE.get(key)
     if hit is not None:
         _CACHE.move_to_end(key)
+        capture.pin(hit[1])
         return hit[1]
     n = int(batch.numel())
     csr = build_csr(torch.arange(n, device=batch.device), batch, n_graphs, n_src=n)
@@ -45,6 +47,7 @@ def segment_reduce(x: torch.Tensor, batch: torch.Tensor, n_graphs: Optional[int]
     if x.dim() != 2 or batch.dim() != 1 or batch.numel() != x.size(0):
         raise ValueError("x must be [N, F] and batch [N]")
     if n_graphs is None:
+        capture.guard("a readout without its graph count (int(batch.max()) reads back)", "pass n_graphs / size")
         n_graphs = int(batch.max()) + 1 if batch.numel() else 0
     return pna_aggregate(at_boundary(x), batch_csr(batch, n_graphs), [reduce], ["identity"], _UNIT)
 
@@ -67,6 +70,7 @@ def _graph_batch(g, device) -> tuple:
     sizes = torch.as_tensor(sizes, dtype=torch.long)
     cached = getattr(g, "_pna_b200_batch", None)
     if cached is None or cached.device != device:
+        capture.guard("the node-to-graph index of this batched graph (a host-to-device copy)")
         cached = torch.repeat_interleave(torch.arange(sizes.numel()), sizes).to(device)
         try:
             g._pna_b200_batch = cached
