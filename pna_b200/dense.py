@@ -31,11 +31,11 @@ once).  Where they deliberately differ from the reference:
 paths, autograd for its gradient) with the kernels' scaler factors of the loop-free row degree.
 
 ``pretrans_layers = L >= 2`` (a ReLU between the layers, so the message is no longer affine): the first layer still
-splits into the node GEMMs A, Bm, b1, and ``pna_edge_mlp_fwd`` (edge_mlp.py) evaluates the rest of the chain once per
-edge of the row CSR, writing M [E, T*F_t] in slot order.  The self-first aggregators read M in CSR order (normalised_mean
-with ``degree_col = row.col``); max/min read the same messages through a third CSR (destination j, sources = the row-slot
-ids of the edges (i, j)), because X[u, v] of the colwise reduction is the message of edge (u, v); ``identity`` runs the
-pretrans MLP on [h_i, h_i] in torch.  Tower widths above 64 raise NotImplementedError.
+splits into the node GEMMs A, Bm, b1 (packed as for the tower layers, towers.py), and ``pna_edge_mlp_fwd``
+(edge_mlp.py) evaluates the rest of the chain once per edge of the row CSR, writing M [E, T*F_t] in slot order.  The
+self-first aggregators read M in CSR order (normalised_mean with ``degree_col = row.col``); max/min read the same
+messages through a third CSR (destination j, sources = the row-slot ids of the edges (i, j)), because X[u, v] of the
+colwise reduction is the message of edge (u, v); ``identity`` runs the pretrans MLP on [h_i, h_i] in torch.  Tower widths above 64 raise NotImplementedError.
 Under ``torch.autocast("cuda")`` A and Bm reach the kernel at the boundary (DESIGN section 2): bf16 ones run
 ``pna_edge_msg_fwd_bf16`` (no edge term, pitch F_t: the arithmetic of ``pna_edge_mlp_fwd``), fp16 ones are upcast to fp32.
 """
@@ -49,6 +49,7 @@ from .csr import build_csr, tensor_version
 from .edge_mlp import edge_mlp
 from . import _lib, capture
 from .nn_blocks import FCLayer, MLP
+from .towers import first_layer_pack, hidden_pack
 
 _SELF_FIRST = ("mean", "std", "sum", "var", "moment3", "moment4", "moment5", "softmax", "softmin", "normalised_mean")
 _MOMENTS = ("moment3", "moment4", "moment5")
@@ -144,13 +145,8 @@ class PNALayer(nn.Module):
     def _halves(self, h):
         """A = h W_first^T, Bm = h W_second^T (+ bias folded where it is gathered), first/second = cat order."""
         it = self.input_tower
-        lins = [tw.pretrans.fully_connected[0].linear for tw in self.towers]
-        Wa, Wb = [l.weight[:, :it] for l in lins], [l.weight[:, it:] for l in lins]
-        b = torch.cat([l.bias for l in lins])
-        if self.divide_input and len(lins) > 1:
-            Wa, Wb = torch.block_diag(*Wa), torch.block_diag(*Wb)
-        else:
-            Wa, Wb = torch.cat(Wa, 0), torch.cat(Wb, 0)
+        Wa, Wb, b, _ = first_layer_pack([tw.pretrans.fully_connected[0].linear for tw in self.towers], it, 0, it,
+                                        self.divide_input)
         return h @ Wa.t(), h @ Wb.t(), b
 
     def _columns(self, width, a2, device):
@@ -176,71 +172,59 @@ class PNALayer(nn.Module):
         graphs = dense_graphs(adj, self.self_loop)
         h = input.reshape(B * N, Fin)
         T = len(self.towers)
-        if not self.towers[0].pretrans.is_single_affine():
-            return self._forward_edge_mlp(h, graphs, B, N)
-        A, Bm, b = self._halves(h)
         a1 = [a if a in _SELF_FIRST else "_skip" for a in self.aggregators]
         a2 = [a if a in _NBR_FIRST else "_skip" for a in self.aggregators]
+        nbr = any(a != "_skip" for a in a2)
         common = dict(towers=T, self_feat=h, self_divided=self.divide_input, relu_var=True,
                       scaler_degree=graphs.scaler_degree)
-        need_grad = torch.is_grad_enabled() and (h.requires_grad or any(p.requires_grad for p in self.parameters()))
-        both = any(a != "_skip" for a in a2) and any(a != "_skip" for a in a1)
-        if not need_grad:
-            # mean/std: message = W_first h_v + W_second h_u + b, neighbours u from row v of adj
-            out = aggregate_forward(Bm + b, graphs.row, a1, self.scalers, self.avg_d, row_bias=A, **common)
-            # max/min: message = W_first h_u + W_second h_v + b, neighbours u from column v of adj; fills the skipped slots
-            if any(a != "_skip" for a in a2):
-                aggregate_forward(A + b, graphs.colwise, a2, self.scalers, self.avg_d, row_bias=Bm, out=out, **common)
+        if not self.towers[0].pretrans.is_single_affine():
+            out, out2, x_id = self._forward_edge_mlp(h, graphs, a1, a2, nbr, common)
         else:
-            # training (multitask_benchmark/util/train.py:148): two differentiable calls, columns merged by a mask
-            out = pna_aggregate(Bm + b, graphs.row, a1, self.scalers, self.avg_d, row_bias=A, **common)
-            if any(a != "_skip" for a in a2):
-                out2 = pna_aggregate(A + b, graphs.colwise, a2, self.scalers, self.avg_d, row_bias=Bm, **common)
-                out = torch.where(self._columns(out.size(1), a2, h.device), out2, out) if both else out2
+            A, Bm, b = self._halves(h)
+            out2, x_id = None, lambda: A + Bm + b
+            if not (torch.is_grad_enabled() and (h.requires_grad or any(p.requires_grad for p in self.parameters()))):
+                # mean/std: message = W_first h_v + W_second h_u + b, neighbours u from row v of adj
+                out = aggregate_forward(Bm + b, graphs.row, a1, self.scalers, self.avg_d, row_bias=A, **common)
+                # max/min: message = W_first h_u + W_second h_v + b, neighbours u from column v of adj; fills the
+                # skipped slots
+                if nbr:
+                    aggregate_forward(A + b, graphs.colwise, a2, self.scalers, self.avg_d, row_bias=Bm, out=out, **common)
+            else:
+                # training (multitask_benchmark/util/train.py:148): two differentiable calls, columns merged by a mask
+                out = pna_aggregate(Bm + b, graphs.row, a1, self.scalers, self.avg_d, row_bias=A, **common)
+                if nbr:
+                    out2 = pna_aggregate(A + b, graphs.colwise, a2, self.scalers, self.avg_d, row_bias=Bm, **common)
+        if out2 is not None:
+            both = any(a != "_skip" for a in a1)
+            out = torch.where(self._columns(out.size(1), a2, h.device), out2, out) if both else out2
         if "identity" in self.aggregators:
             # X_ii = pretrans([h_i, h_i]) per tower, in every scaler's slot; autograd carries its gradient
             ident = [a if a == "identity" else "_skip" for a in self.aggregators]
-            out = torch.where(self._columns(out.size(1), ident, h.device), self._identity_block(A + Bm + b, graphs), out)
+            out = torch.where(self._columns(out.size(1), ident, h.device), self._identity_block(x_id(), graphs), out)
         # both calls scale with the ROW degree D = adj.sum(-1) of the loop-free adjacency (scaler_degree), as
         # models/pytorch/pna/scalers.py:13,21 does, whatever edge set the aggregators reduced over
         out = out.view(B * N, T, -1)
         y = torch.cat([tw.posttrans(out[:, t]) for t, tw in enumerate(self.towers)], dim=1)
         return self.mixing_network(y).view(B, N, -1)
 
-    def _forward_edge_mlp(self, h, graphs, B, N):
-        """pretrans_layers >= 2: per-edge messages from pna_edge_mlp_fwd (module docstring), then the same aggregation,
-        scalers, posttrans and mixing as the affine path."""
-        T = len(self.towers)
-        mlps = [tw.pretrans.fully_connected for tw in self.towers]
+    def _forward_edge_mlp(self, h, graphs, a1, a2, nbr, common):
+        """pretrans_layers >= 2: per-edge messages from pna_edge_mlp_fwd (module docstring) and their aggregation.  Returns
+        the self-first aggregate, the neighbour-first one (None without max/min) and a callable giving the identity
+        block's pretrans([h_i, h_i]); ``forward`` merges them as on the affine path."""
         if not all(tw.pretrans.is_linear_relu() for tw in self.towers):
             raise NotImplementedError("dense PNALayer: the edge-MLP kernel takes Linear/ReLU pretrans layers only")
         A, Bm, b1 = self._halves(h)
-        A, Bm = at_boundary(A), at_boundary(Bm)
-        W = torch.stack([torch.stack([fcs[k].linear.weight for fcs in mlps]) for k in range(1, len(mlps[0]))])
-        bW = torch.stack([torch.stack([fcs[k].linear.bias for fcs in mlps]) for k in range(1, len(mlps[0]))])
-        M = edge_mlp(A, Bm, b1, W, bW, graphs.row, T)
-        a1 = [a if a in _SELF_FIRST else "_skip" for a in self.aggregators]
-        a2 = [a if a in _NBR_FIRST else "_skip" for a in self.aggregators]
-        common = dict(towers=T, self_feat=h, self_divided=self.divide_input, relu_var=True,
-                      scaler_degree=graphs.scaler_degree)
+        W, bW = hidden_pack([[fc.linear for fc in tw.pretrans.fully_connected] for tw in self.towers])
+        M = edge_mlp(at_boundary(A), at_boundary(Bm), b1, W, bW, graphs.row, len(self.towers))
         # self first: row i reads the messages of its own slots; normalised_mean weighs slot s with D of col[s]
         dcol = graphs.row.col if "normalised_mean" in self.aggregators else None
         out = pna_aggregate(M, graphs.row, a1, self.scalers, self.avg_d, messages_in_csr_order=True, degree_col=dcol,
                             **common)
-        if any(a != "_skip" for a in a2):
-            # neighbour first: node v reduces X[u, v] = M[slot of edge (u, v)] over u
-            out2 = pna_aggregate(M, graphs.pairs, a2, self.scalers, self.avg_d, **common)
-            both = any(a != "_skip" for a in a1)
-            out = torch.where(self._columns(out.size(1), a2, h.device), out2, out) if both else out2
-        if "identity" in self.aggregators:
-            it = self.input_tower
-            xs = [h[:, t * it:(t + 1) * it] if self.divide_input else h for t in range(T)]
-            x_id = torch.cat([tw.pretrans(torch.cat([x, x], 1)) for x, tw in zip(xs, self.towers)], 1)
-            ident = [a if a == "identity" else "_skip" for a in self.aggregators]
-            out = torch.where(self._columns(out.size(1), ident, h.device), self._identity_block(x_id, graphs), out)
-        out = out.view(B * N, T, -1)
-        y = torch.cat([tw.posttrans(out[:, t]) for t, tw in enumerate(self.towers)], dim=1)
-        return self.mixing_network(y).view(B, N, -1)
+        # neighbour first: node v reduces X[u, v] = M[slot of edge (u, v)] over u
+        out2 = pna_aggregate(M, graphs.pairs, a2, self.scalers, self.avg_d, **common) if nbr else None
+        it = self.input_tower
+        xs = [h[:, t * it:(t + 1) * it] if self.divide_input else h for t in range(len(self.towers))]
+        return out, out2, lambda: torch.cat([tw.pretrans(torch.cat([x, x], 1)) for x, tw in zip(xs, self.towers)], 1)
 
     def _identity_block(self, x_id, graphs):
         """[B*N, T * (1 + S*A) * F_t]: x_id's tower slice times each scaler's factor in every (scaler, aggregator) slot; the

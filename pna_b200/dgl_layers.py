@@ -13,7 +13,8 @@ pretrans layer they are affine and never built (two node GEMMs and the aggregati
 ``ef`` against every tower's edge columns, and the rest of the pretrans MLP per edge.  The towers' ``pretrans`` run in
 torch on gathered rows only for inputs the kernel does not take: dtypes other than float32, ``pretrans_layers > 1`` with
 a tower width above 64, pretrans stacks that are not plain Linear / ReLU (dropout or batch norm inside), and training
-steps on graphs below ``edge_mlp.FUSED_TRAINING_MIN_EDGES`` edges, where the torch path measured faster.
+steps on graphs below ``edge_mlp.FUSED_TRAINING_MIN_EDGES`` edges, where the torch path measured faster.  This message and
+aggregation path, and the weight packs it caches, are shared with ``PNAConv`` (towers.py).
 
 Under ``torch.autocast("cuda")`` ``PNALayer`` hands its GEMM products to the kernels in ``aggregate.boundary_dtype()``
 (DESIGN section 2): bf16 operands run the bf16 aggregation, messages and compact tower post-linear whatever h's dtype, fp16
@@ -25,14 +26,13 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import _lib, aggregate, capture, padding as pad
-from .aggregate import at_boundary, pna_aggregate, row_scales
-from . import edge_mlp
+from . import padding as pad
+from .aggregate import pna_aggregate, row_scales
 from .edge_mlp import edge_messages
-from .linear import compact_path_ok, post_linear_towers_scaled, towers_compact_pays, towers_path_ok
-from .csr import tensor_version
+from .linear import compact_path_ok, post_linear_towers_scaled
 from .graph import graph_csr
 from .nn_blocks import FCLayer, MLP
+from .towers import TowerLayer
 
 _AGGRS = ("mean", "sum", "max", "min", "std", "var")       # models/dgl/aggregators.py:50-52 minus moment3/4/5
 _SCALERS = ("identity", "amplification", "attenuation")     # models/dgl/scalers.py:22
@@ -90,7 +90,7 @@ class PNATower(nn.Module):
         return F.dropout(h, self.dropout, training=self.training)
 
 
-class PNALayer(nn.Module):
+class PNALayer(TowerLayer, nn.Module):
     """reference pna_layer.py:79-148."""
 
     def __init__(self, in_dim, out_dim, aggregators, scalers, avg_d, dropout, graph_norm, batch_norm, towers=1,
@@ -115,90 +115,38 @@ class PNALayer(nn.Module):
             for _ in range(towers)])
         self.mixing_network = FCLayer(out_dim, out_dim, activation="LeakyReLU")
 
+    n_towers = property(lambda self: len(self.towers))
+    tower_in = property(lambda self: self.input_tower)
+    avg = property(lambda self: self.avg_d)
+
+    # -- what differs from PNAConv on the shared tower path (towers.py) -------------------------------------------------
+    _SRC_FIRST = True                                   # pretrans(cat[src h, dst h, ef]) (pna_layer.py:35-40)
+    _AGG_FLAGS = dict(zero_isolated=True, relu_var=True)
+
+    def _pre_linears(self):
+        return [[fc.linear for fc in tw.pretrans.fully_connected] for tw in self.towers]
+
+    def _post_linears(self):
+        return [tw.posttrans.fully_connected[0].linear for tw in self.towers]
+
+    def _affine(self, e) -> bool:
+        return not self.edge_features and self.towers[0].pretrans.is_single_affine()
+
+    def _fused_layer_ok(self, e, amp: bool) -> bool:
+        """Linear/ReLU pretrans stacks (no dropout or batch norm inside), and ef when edge features are announced."""
+        return ((not self.edge_features or (e is not None and (amp or e.dtype == torch.float32)))
+                and all(tw.pretrans.is_linear_relu() for tw in self.towers))
+
+    def _fused_messages(self, h, csr, e, fp: int):
+        A, Bm, b1, W, bW, C = self._message_operands(h, csr, e if self.edge_features else None)
+        return edge_messages(A, Bm, b1, W, bW, csr, len(self.towers), edge_term=C, pitch=fp)
+
+    def _torch_messages(self, h, csr, e):
+        return self._edge_messages(csr, h, e)
+
     def _tower_input(self, h, t):
         it = self.input_tower
         return h[:, t * it:(t + 1) * it] if self.divide_input else h
-
-    def _affine_terms(self, h, fp):
-        """pretrans(cat[src h, dst h]) = W_s h_src + W_d h_dst + b (pna_layer.py:35-40): V = h W_s^T + b, U = h W_d^T,
-        each tower block padded to fp columns with zero weight rows.  Both come out of ONE GEMM against the packed weight
-        [W_d ; W_s] (block-diagonal per tower with divide_input), which is rebuilt only when a parameter changed (without
-        autograd; with autograd it is part of the graph and rebuilt every call; inside a CUDA graph capture it is rebuilt and
-        not cached, so that a replay follows the weights)."""
-        it = self.input_tower
-        lins = [tw.pretrans.fully_connected[0].linear for tw in self.towers]
-        params = [p_ for l in lins for p_ in (l.weight, l.bias)]
-        key = (fp, tuple(tensor_version(p_) for p_ in params), tuple(p_.data_ptr() for p_ in params))
-        cache = not (torch.is_grad_enabled() and any(p_.requires_grad for p_ in params)) and not capture.capturing()
-        hit = getattr(self, "_uv_pack", None)
-        if cache and hit is not None and hit[0] == key:
-            w_uv, b_uv = hit[1]
-        else:
-            Ws = [pad.expand_weight_rows(l.weight[:, :it], it, fp) for l in lins]
-            Wd = [pad.expand_weight_rows(l.weight[:, it:2 * it], it, fp) for l in lins]
-            b = torch.cat([F.pad(l.bias, (0, fp - it)) for l in lins])
-            if self.divide_input and len(lins) > 1:
-                w_uv = torch.cat([torch.block_diag(*Wd), torch.block_diag(*Ws)], 0)
-            else:
-                w_uv = torch.cat(Wd + Ws, 0)
-            b_uv = torch.cat([torch.zeros_like(b), b])
-            if cache:
-                self._uv_pack = (key, (w_uv, b_uv))
-        uv = torch.addmm(b_uv, h, w_uv.t())
-        half = uv.size(1) // 2
-        return uv[:, :half], uv[:, half:]
-
-    def _fused_messages_ok(self, h, e, n_edges: int) -> bool:
-        """The inputs pna_edge_msg_fwd takes: float32 on the GPU, Linear/ReLU pretrans stacks, and a tower width of at
-        most 64 when there is more than one pretrans layer; with autograd, graphs of at least
-        edge_mlp.FUSED_TRAINING_MIN_EDGES edges (where the kernel path is faster).  Inside autocast the GEMMs make the
-        operands, in the boundary dtype: the dtypes of h and e are not asked, the weights' is."""
-        fc0 = self.towers[0].pretrans.fully_connected
-        amp = aggregate.boundary_dtype() is not None
-        return (edge_mlp.fused_step_pays(n_edges) and h.is_cuda and (amp or h.dtype == torch.float32)
-                and fc0[0].linear.weight.dtype == torch.float32
-                and (not self.edge_features or (e is not None and (amp or e.dtype == torch.float32)))
-                and all(tw.pretrans.is_linear_relu() for tw in self.towers)
-                and (len(fc0) == 1 or self.input_tower <= _lib.EDGE_MLP_MAX_WIDTH))
-
-    def _fused_messages(self, csr, h, e, fp):
-        """[E, T*fp] messages in slot order from pna_edge_msg_fwd, concatenation order [src h, dst h, ef]: Bm = h W[:, :it]^T
-        (source side), A = h W[:, it:2it]^T (destination side), block-diagonal under divide_input; C = ef[perm] W_e^T with
-        W_e every tower's W[:, 2it:] stacked (ef is not split by divide_input); the hidden Linears as [L-1, T, it, it]."""
-        Wd, Ws, b1, We, W, bW = self._message_weights()
-        C = at_boundary(e.index_select(0, csr.perm.long()) @ We.t()) if self.edge_features else None
-        return edge_messages(at_boundary(h @ Wd.t()), at_boundary(h @ Ws.t()), b1, W, bW, csr, len(self.towers), edge_term=C,
-                             pitch=fp)
-
-    def _message_weights(self):
-        """The pretrans weights packed as the kernel takes them; rebuilt only when a parameter changed (without autograd;
-        with autograd the pack is part of the graph and rebuilt every call), as ``_affine_terms``."""
-        it = self.input_tower
-        fcs = [tw.pretrans.fully_connected for tw in self.towers]
-        params = [p_ for f in fcs for fc in f for p_ in (fc.linear.weight, fc.linear.bias)]
-        key = (tuple(tensor_version(p_) for p_ in params), tuple(p_.data_ptr() for p_ in params))
-        cache = not (torch.is_grad_enabled() and any(p_.requires_grad for p_ in params)) and not capture.capturing()
-        hit = getattr(self, "_msg_pack", None)
-        if cache and hit is not None and hit[0] == key:
-            return hit[1]
-        W1 = [f[0].linear.weight for f in fcs]
-        Ws, Wd = [w[:, :it] for w in W1], [w[:, it:2 * it] for w in W1]
-        if self.divide_input and len(fcs) > 1:
-            Wd, Ws = torch.block_diag(*Wd), torch.block_diag(*Ws)
-        else:
-            Wd, Ws = torch.cat(Wd, 0), torch.cat(Ws, 0)
-        b1 = torch.cat([f[0].linear.bias for f in fcs])
-        We = torch.cat([w[:, 2 * it:] for w in W1], 0) if self.edge_features else None
-        L = len(fcs[0])
-        if L > 1:
-            W = torch.stack([torch.stack([f[k].linear.weight for f in fcs]) for k in range(1, L)])
-            bW = torch.stack([torch.stack([f[k].linear.bias for f in fcs]) for k in range(1, L)])
-        else:
-            W = bW = W1[0].new_empty(0)
-        pack = (Wd, Ws, b1, We, W, bW)
-        if cache:
-            self._msg_pack = (key, pack)
-        return pack
 
     def _edge_messages(self, csr, h, e):
         src, dst = csr.col.long(), csr.dst_of_slot
@@ -210,51 +158,19 @@ class PNALayer(nn.Module):
             msgs.append(tw.pretrans(torch.cat(parts, dim=1)))
         return torch.cat(msgs, dim=1)
 
-    def _compact(self, h, fp: int) -> bool:
-        """Compact post path: aggregate with the identity scaler only ([N, T * (1 + A) * fp]) and let
-        pna_linear_towers_scaled_fwd form the scaled copies in registers -- the [N, T * (1 + S*A) * fp] tensor is never
-        written, nor saved for the backward.  Same arithmetic; float32 with more than one scaler, at the kernel's shapes,
-        in training steps on graphs of at least linear.TOWERS_COMPACT_MIN_ROWS rows, where it measured faster."""
-        fc0 = self.towers[0].posttrans.fully_connected[0].linear
-        training = torch.is_grad_enabled() and any(p_.requires_grad for p_ in self.parameters())
-        return fc0.weight.dtype == torch.float32 and fc0.bias is not None and \
-            towers_path_ok(h, len(self.towers), fp, self.output_tower, len(self.scalers)) and \
-            towers_compact_pays(h.size(0), training)
-
     def forward(self, g, h, e, snorm_n):
         h_in = h
         csr = graph_csr(g, h.device)
-        T, it = len(self.towers), self.input_tower
-        fp = pad.padded_width(it, aggregate.boundary_dtype() or h.dtype)      # the kernels' dtype: bf16 pads to 8 columns
-        if fp == it:
-            h_self = h
-        elif self.divide_input:
-            h_self = pad.pad_blocks(h, T, it, fp)
-        else:
-            h_self = pad.pad_cols(h, fp)
-        common = dict(towers=T, self_feat=h_self, self_divided=self.divide_input, zero_isolated=True, relu_var=True)
-        compact = self._compact(h, fp)
-        scalers = ["identity"] if compact else self.scalers
-        if not self.edge_features and self.towers[0].pretrans.is_single_affine():
-            U, V = (at_boundary(t) for t in self._affine_terms(h, fp))
-            agg = pna_aggregate(V, csr, self.aggregators, scalers, self.avg_d, row_bias=U, **common)
-        else:
-            if self._fused_messages_ok(h, e, csr.n_edges):
-                msgs = self._fused_messages(csr, h, e, fp)
-            else:
-                msgs = at_boundary(pad.pad_blocks(self._edge_messages(csr, h, e), T, it, fp))
-            agg = pna_aggregate(msgs, csr, self.aggregators, scalers, self.avg_d, messages_in_csr_order=True, **common)
-        blocks = 1 + len(self.aggregators) * len(self.scalers)
+        fp = self._tower_pitch(h)
+        agg, compact = self._aggregate_towers(h, csr, e, fp, self._self_features(h, fp))
         if compact:
-            # compact post path: [N, T, (1 + A) * fp] aggregate, every tower's first posttrans Linear in one kernel that
-            # forms the scaled copies in registers; the rest of each tower's posttrans and norms on its output_tower slice
-            lins = [tw.posttrans.fully_connected[0].linear for tw in self.towers]
-            w0 = torch.stack([pad.expand_weight_cols(l.weight, blocks, it, fp) for l in lins])
-            y = post_linear_towers_scaled(agg, row_scales(csr, self.scalers, self.avg_d), w0, torch.stack([l.bias for l in lins]))
+            # the rest of each tower's posttrans and norms on its output_tower slice of the towers' first posttrans Linear
+            y = post_linear_towers_scaled(agg, row_scales(csr, self.scalers, self.avg_d), *self._post_weights(fp))
             ot = self.output_tower
             h_cat = torch.cat([tw.finish_linear(y[:, t * ot:(t + 1) * ot], snorm_n) for t, tw in enumerate(self.towers)], dim=1)
         else:
-            agg = agg.view(h.size(0), T, -1)                              # [N, T, (1 + S*A) * fp] = cat([h_t, reduced])
+            blocks = 1 + len(self.aggregators) * len(self.scalers)
+            agg = agg.view(h.size(0), len(self.towers), -1)                # [N, T, (1 + S*A) * fp] = cat([h_t, reduced])
             h_cat = torch.cat([tw.finish(agg[:, t], snorm_n, blocks, fp) for t, tw in enumerate(self.towers)], dim=1)
         h_out = self.mixing_network(h_cat)
         if self.residual:

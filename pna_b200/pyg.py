@@ -4,6 +4,7 @@ Drop-in for reference ``models/pytorch_geometric/pna.py``: same constructor argu
 ``forward(x, edge_index, edge_attr=None)``, same parameter names (``pre_nns.{t}.{k}``, ``post_nns.{t}.{k}``,
 ``lin``, ``edge_encoder``; ``post_nn.{k}`` for the simple layer) so reference ``state_dict``s load unchanged.
 torch_geometric is NOT needed: ``MessagePassing.propagate`` (gather + scatter) is what the kernel replaces.
+``PNAConv`` shares its weight packs, messages and aggregation with the DGL ``PNALayer`` (towers.py).
 """
 from __future__ import annotations
 
@@ -13,12 +14,12 @@ import torch
 from torch import Tensor
 from torch.nn import Linear, Module, ModuleList, ReLU, Sequential
 
-from . import _lib, aggregate, capture, padding as pad
-from .aggregate import at_boundary, avg_deg_from_histogram, pna_aggregate, row_scales
-from . import edge_mlp
+from . import capture, padding as pad
+from .aggregate import avg_deg_from_histogram, pna_aggregate, row_scales
 from .edge_mlp import edge_messages
-from .linear import compact_path_ok, linear_tf32x3, post_linear, post_linear_scaled, post_linear_towers_scaled, towers_compact_pays, towers_path_ok
-from .csr import CSRGraph, csr_from_edge_index, tensor_version
+from .linear import compact_path_ok, linear_tf32x3, post_linear, post_linear_scaled, post_linear_towers_scaled
+from .csr import CSRGraph, csr_from_edge_index
+from .towers import TowerLayer, cached
 
 _AGGRS = ("sum", "mean", "min", "max", "var", "std")          # aggregators.py:35-42
 _SCALERS = ("identity", "amplification", "attenuation", "linear", "inverse_linear")  # scalers.py:32-38
@@ -158,7 +159,7 @@ class PNAConvSimple(Module):
         return f"{self.__class__.__name__}({self.in_channels}, {self.out_channels})"
 
 
-class PNAConv(Module):
+class PNAConv(TowerLayer, Module):
     """reference pna.py:17-164.  Towers, pre-MLP on [x_i || x_j (|| e)], aggregation, post-MLP on [x || agg], lin.
 
     With ``pre_layers == 1`` and no edge features the message is affine in (x_i, x_j):
@@ -224,92 +225,42 @@ class PNAConv(Module):
             _reset(nn)
         self.lin.reset_parameters()
 
-    # -- weights in the layout the forward pass consumes ------------------------------------------------------------------
+    n_towers = property(lambda self: self.towers)
+    tower_in = property(lambda self: self.F_in)
+    avg = property(lambda self: self.avg_deg)
+
+    # -- what differs from the DGL layer on the shared tower path (towers.py) ------------------------------------------
+    def _pre_linears(self):
+        return [list(nn)[0::2] for nn in self.pre_nns]           # the Linears of each tower (ReLU between them)
+
+    def _post_linears(self):
+        return [nn[0] for nn in self.post_nns]
+
+    def _affine(self, edge_attr) -> bool:
+        return edge_attr is None and self.pre_layers == 1 and self.edge_dim is None
+
+    def _fused_layer_ok(self, edge_attr, amp: bool) -> bool:
+        return (edge_attr is None) == (self.edge_dim is None)
+
     def _prepared(self, Fp: int):
-        """The towers' weights packed once per parameter version instead of once per call:
-          w_uv [2*T*Fp, in], b_uv  -- rows [0, T*Fp) give U = x W_i^T (destination side), rows [T*Fp, 2*T*Fp) give
-                                      V = x W_j^T + b (source side): ONE node-level GEMM for both (pna.py:94,147-149);
-                                      divide_input: tower t only sees its own F_in input columns (block-diagonal);
-          w_post [T, F_out, (1+S*A)*Fp], b_post [T, F_out] -- first post Linear of every tower with zero columns at the pad
-                                      positions: ONE batched GEMM over all towers (pna.py:132).
-        With autograd enabled the pack is rebuilt every call (it is part of the graph); otherwise it is cached, except
-        inside a CUDA graph capture, where the packing is captured so that a replay follows the weights."""
+        """U|V and the first post Linears as one cached pack (``towers.cached``), w_uv, b_uv, w_post, b_post: every path of
+        this layer that reads one reads the other.  U | V = x w_uv^T + b_uv is ONE node-level GEMM (pna.py:94,147-149), the
+        first post Linear of every tower ONE batched GEMM or one tower kernel (pna.py:132)."""
         params = [p_ for nn in list(self.pre_nns) + list(self.post_nns) for p_ in nn[0].parameters()]
-        key = (Fp, tuple(tensor_version(p_) for p_ in params), tuple(p_.data_ptr() for p_ in params))
-        cache = (torch.is_grad_enabled() is False or not any(p_.requires_grad for p_ in params)) and not capture.capturing()
-        if cache and getattr(self, "_prep", None) is not None and self._prep[0] == key:
-            return self._prep[1]
-        T, Fi = self.towers, self.F_in
-        Wi = [pad.expand_weight_rows(nn[0].weight[:, :Fi], Fi, Fp) for nn in self.pre_nns]
-        Wj = [pad.expand_weight_rows(nn[0].weight[:, Fi:2 * Fi], Fi, Fp) for nn in self.pre_nns]
-        b = torch.cat([torch.nn.functional.pad(nn[0].bias, (0, Fp - Fi)) for nn in self.pre_nns])
-        if self.divide_input and T > 1:
-            w_uv = torch.cat([torch.block_diag(*Wi), torch.block_diag(*Wj)], 0)
-        else:
-            w_uv = torch.cat(Wi + Wj, 0)
-        b_uv = torch.cat([torch.zeros_like(b), b])
-        blocks = 1 + len(self.aggregators) * len(self.scalers)
-        w_post = torch.stack([pad.expand_weight_cols(nn[0].weight, blocks, Fi, Fp) for nn in self.post_nns])
-        b_post = torch.stack([nn[0].bias for nn in self.post_nns])
-        prep = (w_uv, b_uv, w_post, b_post)
-        if cache:
-            self._prep = (key, prep)
-        return prep
+        return cached(self, "_prep", Fp, params, lambda: self._first_layer(Fp, joined=True) + self._post_pack(Fp))
 
-    # -- message side ---------------------------------------------------------------------------------------------
-    def _affine_terms(self, x: Tensor, Fp: int):
-        """U = x W_i^T (destination side), V = x W_j^T + b (source side), both [N, T*Fp] -- two halves of one GEMM result;
-        Fp >= F_in pads every tower block with zero features (zero weight rows: the GEMM writes them)."""
-        w_uv, b_uv = self._prepared(Fp)[:2]
-        uv = torch.addmm(b_uv, x, w_uv.t())
-        h = uv.size(1) // 2
-        return uv[:, :h], uv[:, h:]
+    def _uv_weights(self, Fp: int):
+        return self._prepared(Fp)[:2]
 
-    def _fused_messages_ok(self, x: Tensor, edge_attr: Optional[Tensor], n_edges: int) -> bool:
-        """The inputs pna_edge_msg_fwd takes: float32 on the GPU, and a tower width of at most 64 with pre_layers > 1;
-        with autograd, graphs of at least edge_mlp.FUSED_TRAINING_MIN_EDGES edges (where the kernel path is faster).
-        Inside autocast the GEMMs make the operands, in the boundary dtype: x's own dtype is not asked, the weights' is."""
-        x_ok = x.dtype == torch.float32 or aggregate.boundary_dtype() is not None
-        return (edge_mlp.fused_step_pays(n_edges) and x.is_cuda and x_ok and self.pre_nns[0][0].weight.dtype == torch.float32
-                and (edge_attr is None) == (self.edge_dim is None)
-                and (self.pre_layers == 1 or self.F_in <= _lib.EDGE_MLP_MAX_WIDTH))
+    def _post_weights(self, Fp: int):
+        return self._prepared(Fp)[2:]
 
-    def _fused_messages(self, x: Tensor, csr: CSRGraph, edge_attr: Optional[Tensor], Fp: int) -> Tensor:
-        """[E, T*Fp] messages in slot order from pna_edge_msg_fwd: A = x W_i^T (x_i side), Bm = x W_j^T (x_j side),
-        block-diagonal under divide_input; C = edge_encoder(edge_attr)[perm] W_e^T with W_e the towers' W[:, 2F:3F]
-        stacked (one GEMM); the hidden Linears stacked as [L-1, T, F, F]."""
-        Wi, Wj, b1, We, W, bW = self._message_weights()
-        C = None
-        if edge_attr is not None:
-            C = at_boundary(self.edge_encoder(edge_attr).index_select(0, csr.perm.long()) @ We.t())
-        return edge_messages(at_boundary(x @ Wi.t()), at_boundary(x @ Wj.t()), b1, W, bW, csr, self.towers, edge_term=C, pitch=Fp)
+    def _fused_messages(self, x, csr, edge_attr, Fp: int):
+        A, Bm, b1, W, bW, C = self._message_operands(x, csr, None if edge_attr is None else self.edge_encoder(edge_attr))
+        return edge_messages(A, Bm, b1, W, bW, csr, self.towers, edge_term=C, pitch=Fp)
 
-    def _message_weights(self):
-        """The pre_nns weights packed as the kernel takes them, cached per parameter version like ``_prepared``."""
-        T, Fi = self.towers, self.F_in
-        lins = [list(nn)[0::2] for nn in self.pre_nns]           # the Linears of each tower (ReLU between them)
-        params = [p_ for l in lins for lin in l for p_ in lin.parameters()]
-        key = (tuple(tensor_version(p_) for p_ in params), tuple(p_.data_ptr() for p_ in params))
-        cache = (torch.is_grad_enabled() is False or not any(p_.requires_grad for p_ in params)) and not capture.capturing()
-        if cache and getattr(self, "_msg_pack", None) is not None and self._msg_pack[0] == key:
-            return self._msg_pack[1]
-        W1 = [l[0].weight for l in lins]
-        Wi, Wj = [w[:, :Fi] for w in W1], [w[:, Fi:2 * Fi] for w in W1]
-        if self.divide_input and T > 1:
-            Wi, Wj = torch.block_diag(*Wi), torch.block_diag(*Wj)
-        else:
-            Wi, Wj = torch.cat(Wi, 0), torch.cat(Wj, 0)
-        b1 = torch.cat([l[0].bias for l in lins])
-        We = torch.cat([w[:, 2 * Fi:3 * Fi] for w in W1], 0) if self.edge_dim is not None else None
-        if self.pre_layers > 1:
-            W = torch.stack([torch.stack([l[k].weight for l in lins]) for k in range(1, self.pre_layers)])
-            bW = torch.stack([torch.stack([l[k].bias for l in lins]) for k in range(1, self.pre_layers)])
-        else:
-            W = bW = W1[0].new_empty(0)
-        pack = (Wi, Wj, b1, We, W, bW)
-        if cache:
-            self._msg_pack = (key, pack)
-        return pack
+    def _torch_messages(self, x, csr, edge_attr):
+        return self._messages_in_slot_order(x, csr, edge_attr)
 
     def _messages_in_slot_order(self, x: Tensor, csr: CSRGraph, edge_attr: Optional[Tensor]) -> Tensor:
         """General path (edge features or pre_layers > 1): pna.py:137-150 evaluated on CSR-ordered edges."""
@@ -328,18 +279,16 @@ class PNAConv(Module):
     # -- inference on the tensor cores: every GEMM of the layer through pna_linear_fwd (3xTF32, fp32-accurate) --------------
     def _tensor_core_pack(self, Fp: int):
         """Weights of the three dense steps at the shapes pna_linear_fwd takes (K a multiple of 32, 64/128/256 outputs), zero
-        padded; cached per parameter version like `_prepared`:
+        padded; cached per parameter version (``towers.cached``):
           U|V      [N, in -> K1] x [O1, K1]:  O1 >= 2*T*Fp rows (U block, V block, zero rows), bias only on the V block;
           towers   [N, T*W -> K2] x [O2, K2]: BLOCK-DIAGONAL -- output columns t*F_out.. read only tower t's W input
                    columns, so one launch does the first post Linear of every tower (pna.py:132) and its output is already
                    the concatenation torch.cat(outs, dim=1) of pna.py:134;
-          lin      [N, O2] x [O3, O2]:        the final Linear (pna.py:135) on that buffer; pad columns meet zero weights.
-        Inside a CUDA graph capture the pack is built every call and not cached (``_prepared``)."""
+          lin      [N, O2] x [O3, O2]:        the final Linear (pna.py:135) on that buffer; pad columns meet zero weights."""
         params = [p_ for nn in list(self.pre_nns) + list(self.post_nns) for p_ in nn[0].parameters()] + list(self.lin.parameters())
-        key = ("tc", Fp, tuple(tensor_version(p_) for p_ in params), tuple(p_.data_ptr() for p_ in params))
-        cache = not capture.capturing()
-        if cache and getattr(self, "_tc", None) is not None and self._tc[0] == key:
-            return self._tc[1]
+        return cached(self, "_tc", ("tc", Fp), params, lambda: self._build_tensor_core_pack(Fp))
+
+    def _build_tensor_core_pack(self, Fp: int):
         up32 = lambda v: (v + 31) // 32 * 32
         pick = lambda v: 64 if v <= 64 else 128 if v <= 128 else 256
         T, Fo = self.towers, self.F_out
@@ -358,10 +307,7 @@ class PNAConv(Module):
         O3 = pick(self.out_channels)
         w3 = torch.zeros((O3, O2), dtype=dt, device=dev); w3[: self.out_channels, : T * Fo] = self.lin.weight
         b3 = torch.zeros(O3, dtype=dt, device=dev); b3[: self.out_channels] = self.lin.bias
-        pack = dict(K1=K1, w1=w1, b1=b1, K2=K2, w2=w2, b2=b2, w3=w3, b3=b3)
-        if cache:
-            self._tc = (key, pack)
-        return pack
+        return dict(K1=K1, w1=w1, b1=b1, K2=K2, w2=w2, b2=b2, w3=w3, b3=b3)
 
     def _tensor_core_ok(self, x: Tensor, edge_attr, Fp: int) -> bool:
         import os
@@ -391,52 +337,23 @@ class PNAConv(Module):
         h = linear_tf32x3(buf, tc["w2"], tc["b2"])                                               # [N, O2] = cat over towers | 0
         return linear_tf32x3(h, tc["w3"], tc["b3"])[:, : self.out_channels]
 
-    def _compact(self, x: Tensor, Fp: int) -> bool:
-        """Compact post path (taken wherever _forward_tensor_cores is not): aggregate with the identity scaler only
-        ([N, T*(1 + A)*Fp]) and let pna_linear_towers_scaled_fwd form the scaled copies in registers -- the
-        [N, T*(1 + S*A)*Fp] tensor is never written, nor saved for the backward.  Same arithmetic.  Training steps on
-        graphs of at least linear.TOWERS_COMPACT_MIN_ROWS rows, where it measured faster."""
-        w = self.post_nns[0][0].weight
-        training = torch.is_grad_enabled() and any(p_.requires_grad for p_ in self.parameters())
-        return (w.dtype == torch.float32 and towers_path_ok(x, self.towers, Fp, self.F_out, len(self.scalers))
-                and towers_compact_pays(x.size(0), training))
-
     def forward(self, x: Tensor, edge_index: Tensor, edge_attr: Optional[Tensor] = None, *,
                 deg: Optional[Tensor] = None, csr: Optional[CSRGraph] = None) -> Tensor:
         csr = _resolve_csr(x, edge_index, csr)
-        T, Fi = self.towers, self.F_in
-        Fp = pad.padded_width(Fi, aggregate.boundary_dtype() or x.dtype)      # the kernels' dtype: bf16 pads to 8 columns
-        # self features at the (possibly padded) tower width
-        if Fp == Fi:
-            x_self = x
-        elif self.divide_input:
-            x_self = pad.pad_blocks(x, T, Fi, Fp)
-        else:
-            x_self = pad.pad_cols(x, Fp)
+        T = self.towers
+        Fp = self._tower_pitch(x)
+        x_self = self._self_features(x, Fp)
         if self._tensor_core_ok(x, edge_attr, Fp):
             return self._forward_tensor_cores(x, csr, x_self, Fp)
-        common = dict(towers=T, self_feat=x_self, self_divided=self.divide_input)
-        compact = self._compact(x, Fp)
-        scalers = ["identity"] if compact else self.scalers
-        if edge_attr is None and self.pre_layers == 1 and self.edge_dim is None:
-            U, V = (at_boundary(t) for t in self._affine_terms(x, Fp))
-            out = pna_aggregate(V, csr, self.aggregators, scalers, self.avg_deg, row_bias=U, **common)
-        else:
-            if self._fused_messages_ok(x, edge_attr, csr.n_edges):
-                msgs = self._fused_messages(x, csr, edge_attr, Fp)
-            else:
-                msgs = at_boundary(pad.pad_blocks(self._messages_in_slot_order(x, csr, edge_attr), T, Fi, Fp))
-            out = pna_aggregate(msgs, csr, self.aggregators, scalers, self.avg_deg, messages_in_csr_order=True,
-                                **common)
-        w_post, b_post = self._prepared(Fp)[2:]
+        out, compact = self._aggregate_towers(x, csr, edge_attr, Fp, x_self)
         if compact:
-            # [N, T*(1 + A)*Fp] -> first post Linear of every tower in one kernel (the scaled copies in its registers),
-            # already the concatenation over the towers (pna.py:134)
-            h = post_linear_towers_scaled(out, row_scales(csr, self.scalers, self.avg_deg), w_post, b_post)
+            # the first post Linear of every tower in one kernel, already the concatenation over the towers (pna.py:134)
+            h = post_linear_towers_scaled(out, row_scales(csr, self.scalers, self.avg_deg), *self._post_weights(Fp))
             if len(self.post_nns[0]) > 1:
                 Fo = self.F_out
                 h = torch.cat([self._rest(nn, h[:, t * Fo:(t + 1) * Fo]) for t, nn in enumerate(self.post_nns)], dim=1)
             return self.lin(h)
+        w_post, b_post = self._post_weights(Fp)
         out = out.view(x.size(0), T, -1)                       # [N, T, (1 + S*A) * Fp]  (pna.py:131)
         # first post Linear of all towers: one batched GEMM on the [N, T, W] view (tower = batch, no copy of the big tensor)
         h = torch.baddbmm(b_post.unsqueeze(1), out.transpose(0, 1), w_post.transpose(1, 2))      # [T, N, F_out]
