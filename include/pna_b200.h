@@ -305,6 +305,36 @@ int pna_aggregate_bwd_slots(const pna_agg_t* desc, const void* grad_out, int64_t
                             float* grad_slots, int64_t ld_grad_slots, float* grad_row_bias, int64_t ld_grad_row_bias,
                             pna_stream_t stream);
 
+/* ---- slot weights: a weighted adjacency (the dense reference's real-valued adj; GCN-normalised or attention weights) ----
+ * The three calls below are pna_aggregate_fwd / pna_aggregate_bwd / pna_aggregate_bwd_slots with two more inputs (both
+ * optional; with both NULL each is exactly the call it extends):
+ *   slot_weight      fp32 [n_edges] in CSR slot order: a real weight w_s per slot.
+ *   scaler_degree_f  fp32 [n_rows]: a real-valued degree D_i for the scalers (amplification log(D+1)/avg_log, attenuation
+ *                    D ? avg_log/log(D+1) : 1, linear D/avg_lin, inverse_linear D ? avg_lin/D : 1); takes precedence over
+ *                    desc->scaler_degree.  With slot_weight NULL every weight is 1.
+ * For row i with slots s, W_i = fp32 sum of w_s in slot order (split rows: over all their slots in slot order too), every
+ * product rounded:
+ *   sum  = fp32 sum of fl(m_s * w_s) in slot order (split rows: chunk sums added in chunk order)
+ *   mean = sum / W_i (correctly rounded);  var = fl(Q / W_i) - fl(mean * mean),  Q = sum of fl(fl(m_s * m_s) * w_s)
+ *   std  = sqrt(max(var, 0) + 1e-5);  var is clamped at 0 with PNA_FLAG_RELU_VAR, as without weights
+ *   min / max over the slots with w_s > 0 of the UNWEIGHTED m_s (the dense reference's adj > 0 mask), 0 when there is none
+ * A row without slots gives what it gives without weights; a row whose weights sum to exactly 0 gets the IEEE quotient.
+ * Gradient of slot s: fl(w_s * fl(c0 + c1 * m_s)) + the routed min / max terms, c0 and c1 the unweighted coefficients with
+ * the degree replaced by W_i (so all-ones weights give the unweighted bits on rows below the split threshold).  No gradient
+ * with respect to the weights.  Aggregators: sum / mean / min / max / var / std (and PNA_AGGR_SKIP); any other aggregator,
+ * peer_gathered and row_ids return PNA_ERR_UNSUPPORTED before anything is enqueued.  The weighted calls have no coefficient
+ * or peer-memory form.  Every other argument, check and scratch contract is the extended call's.  Rounding order:
+ * pna_b200/csrc/pna_aggregate_adj_weight.cuh */
+int pna_aggregate_fwd_weighted(const pna_agg_t* desc, const float* slot_weight, const float* scaler_degree_f,
+                               pna_stream_t stream);
+int pna_aggregate_bwd_weighted(const pna_agg_t* desc, const float* slot_weight, const float* scaler_degree_f,
+                               const void* grad_out, int64_t ld_grad_out, float* grad_gathered, int64_t ld_grad_gathered,
+                               float* grad_row_bias, int64_t ld_grad_row_bias, pna_stream_t stream);
+int pna_aggregate_bwd_slots_weighted(const pna_agg_t* desc, const float* slot_weight, const float* scaler_degree_f,
+                                     const void* grad_out, int64_t ld_grad_out, int32_t f_begin, int32_t f_count,
+                                     float* grad_slots, int64_t ld_grad_slots, float* grad_row_bias, int64_t ld_grad_row_bias,
+                                     pna_stream_t stream);
+
 /* Step 1 of pna_aggregate_bwd_slots for a peer-memory graph (desc->peer_gathered != NULL, required: PNA_ERR_BAD_ARG
  * otherwise): the source row of slot s is row (col[s] & mask) of rank (col[s] >> peer_shift), read over NVLink as
  * pna_aggregate_fwd reads it.  Same arguments, slab rules and results: grad_slots row s and grad_row_bias are the bits

@@ -19,7 +19,8 @@ CUDA_SOURCES = [os.path.join(_HERE, "csrc", n) for n in
                  "pna_aggregate_bf16_scalar.cu", "pna_aggregate_bwd.cu", "pna_linear.cu", "pna_csr.cu", "pna_peer.cu", "pna_misc.cu",
                  "pna_edge_mlp.cu")]
 CUDA_HEADERS = [os.path.join(_HERE, "csrc", n) for n in ("common.cuh", "pna_aggregate.cuh", "pna_aggregate_impl.cuh",
-                                                                   "pna_aggregate_moments.cuh", "pna_aggregate_weighted.cuh")] + [
+                                                                   "pna_aggregate_moments.cuh", "pna_aggregate_weighted.cuh",
+                                                                   "pna_aggregate_adj_weight.cuh")] + [
     os.path.join(REPO_ROOT, "include", "pna_b200.h")]
 BUILD_DIR = os.path.join(_HERE, "csrc", "build")
 
@@ -53,7 +54,8 @@ EXPORTED_SYMBOLS = ("pna_csr_workspace_bytes", "pna_csr_build", "pna_csr_light_v
                     "pna_linear_bwd_workspace_bytes", "pna_linear_bwd_data", "pna_linear_bwd_weight", "pna_edge_mlp_fwd",
                     "pna_edge_mlp_bwd", "pna_edge_msg_fwd", "pna_edge_msg_bwd", "pna_query", "pna_last_error",
                     "pna_linear_towers_scaled_fwd", "pna_linear_towers_bwd_data", "pna_edge_msg_fwd_bf16", "pna_edge_msg_bwd_bf16",
-                    "pna_linear_towers_scaled_fwd_bf16")
+                    "pna_linear_towers_scaled_fwd_bf16", "pna_aggregate_fwd_weighted", "pna_aggregate_bwd_weighted",
+                    "pna_aggregate_bwd_slots_weighted")
 
 
 class PnaError(RuntimeError):
@@ -183,6 +185,13 @@ def lib() -> C.CDLL:
         L.pna_aggregate_bwd_slots.restype = C.c_int
         L.pna_aggregate_bwd_slots.argtypes = [C.POINTER(AggStruct), C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_void_p, C.c_int64,
                                               C.c_void_p, C.c_int64, C.c_void_p]
+        L.pna_aggregate_fwd_weighted.restype = C.c_int
+        L.pna_aggregate_fwd_weighted.argtypes = [C.POINTER(AggStruct), C.c_void_p, C.c_void_p, C.c_void_p]
+        L.pna_aggregate_bwd_weighted.restype = C.c_int
+        L.pna_aggregate_bwd_weighted.argtypes = [C.POINTER(AggStruct), C.c_void_p, C.c_void_p] + L.pna_aggregate_bwd.argtypes[1:]
+        L.pna_aggregate_bwd_slots_weighted.restype = C.c_int
+        L.pna_aggregate_bwd_slots_weighted.argtypes = [C.POINTER(AggStruct), C.c_void_p, C.c_void_p] + \
+            L.pna_aggregate_bwd_slots.argtypes[1:]
         L.pna_aggregate_bwd_peer_slots.restype = C.c_int
         L.pna_aggregate_bwd_peer_slots.argtypes = L.pna_aggregate_bwd_slots.argtypes
         L.pna_gather_rows.restype = C.c_int

@@ -52,8 +52,8 @@ def _dynamic_tail(csr: CSRGraph) -> bool:
 
 
 def _check_scaler_degree(t: torch.Tensor, n_rows: int, dev) -> torch.Tensor:
-    if t.dtype != torch.int32 or t.device != dev or t.numel() != n_rows or not t.is_contiguous():
-        raise ValueError("scaler_degree must be a contiguous int32 [n_rows] tensor on the same device")
+    if t.dtype not in (torch.int32, torch.float32) or t.device != dev or t.numel() != n_rows or not t.is_contiguous():
+        raise ValueError("scaler_degree must be a contiguous int32 or float32 [n_rows] tensor on the same device")
     return t
 
 
@@ -61,6 +61,34 @@ def _check_degree_col(t: torch.Tensor, n_edges: int, dev) -> torch.Tensor:
     if t.dtype != torch.int32 or t.device != dev or t.numel() != n_edges or not t.is_contiguous():
         raise ValueError("degree_col must be a contiguous int32 [n_edges] tensor on the same device")
     return t
+
+
+def _set_scaler_degree(d, t: torch.Tensor, n_rows: int, dev) -> None:
+    """int32: pna_agg_t.scaler_degree.  float32 (a real-valued degree, the weighted dense adjacency) goes to the weighted
+    entry points instead (:func:`_weights`)."""
+    t = _check_scaler_degree(t, n_rows, dev)
+    if t.dtype == torch.int32:
+        d.scaler_degree = t.data_ptr()
+
+
+# what a call with slot weights (or a float32 scaler degree) takes
+ADJ_WEIGHT_AGGREGATORS = ("sum", "mean", "min", "max", "var", "std", "_skip")
+
+
+def _weights(w: Optional[torch.Tensor], aggregators: Names, scaler_degree: Optional[torch.Tensor], n_edges: int, dev):
+    """(slot_weight, scaler_degree_f) device pointers for pna_aggregate_*_weighted, or None when the call is unweighted.
+    slot_weight: fp32 [E] in CSR slot order.  Weighted calls take the aggregators of ADJ_WEIGHT_AGGREGATORS only (the library
+    returns PNA_ERR_UNSUPPORTED for the others; refused here before anything is enqueued)."""
+    sdf = scaler_degree if scaler_degree is not None and scaler_degree.dtype == torch.float32 else None
+    if w is None and sdf is None:
+        return None
+    bad = [a for a in _names(aggregators) if a not in ADJ_WEIGHT_AGGREGATORS]
+    if bad:
+        raise NotImplementedError(f"slot weights / a real-valued scaler degree take {ADJ_WEIGHT_AGGREGATORS[:-1]} only, "
+                                  f"not {bad}")
+    if w is not None and (w.dtype != torch.float32 or w.device != dev or w.numel() != n_edges or not w.is_contiguous()):
+        raise ValueError("slot_weight must be a contiguous float32 [n_edges] tensor on the same device, in CSR slot order")
+    return _ptr(w), _ptr(sdf)
 
 
 def fold_finalize_enabled() -> bool:
@@ -102,7 +130,7 @@ def aggregate_forward(gathered: torch.Tensor, csr: CSRGraph, aggregators: Names,
                       out: Optional[torch.Tensor] = None, row_ids: Optional[torch.Tensor] = None,
                       skip_light: bool = False, skip_hubs: bool = False, view=None, peer=None,
                       scaler_degree: Optional[torch.Tensor] = None, gather_l1: Optional[bool] = None,
-                      degree_col: Optional[torch.Tensor] = None) -> torch.Tensor:
+                      degree_col: Optional[torch.Tensor] = None, slot_weight: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Run the CUDA aggregation (no autograd).  Returns ``[N, towers * (has_self + S*A) * Ft]``.
 
     gathered : [n_src, F] rows that are gathered through ``csr.col`` (x for PNAConvSimple; V = x W_j^T + b for
@@ -113,6 +141,10 @@ def aggregate_forward(gathered: torch.Tensor, csr: CSRGraph, aggregators: Names,
                ``t*Ft:(t+1)*Ft`` (divide_input=True) or the same ``0:Ft`` (repeat, pna.py:126).
     degree_col: optional int32 [E]: for normalised_mean, the row of this CSR whose degree weighs each slot (in place of
                ``col``) -- what lets it run on messages in CSR order (pna_agg_t.degree_col).
+    scaler_degree: optional [N] degree the scalers see: int32 (pna_agg_t.scaler_degree) or float32, a real-valued degree
+               such as ``adj.sum(-1)`` of a weighted adjacency (pna_aggregate_fwd_weighted's scaler_degree_f).
+    slot_weight: optional float32 [E] weight of every CSR slot (pna_aggregate_fwd_weighted): sum / mean / var / std weigh every
+               message, min / max reduce over the slots of positive weight; a constant (no gradient).
     """
     if "normalised_mean" in _names(aggregators):
         # its weight D_i^(-1/2) D_j^(-1/2) reads the source's degree from the same CSR: every gathered row must be a row of
@@ -179,7 +211,8 @@ def aggregate_forward(gathered: torch.Tensor, csr: CSRGraph, aggregators: Names,
         n_hubs=csr.n_hubs, n_chunks=csr.n_chunks, hub_partials=_ptr(partials), max_degree=int(csr.max_degree),
         row_ids=_ptr(row_ids), n_row_ids=0 if row_ids is None else int(row_ids.numel()))
     if scaler_degree is not None:
-        d.scaler_degree = _check_scaler_degree(scaler_degree, N, dev).data_ptr()
+        _set_scaler_degree(d, scaler_degree, N, dev)
+    weights = _weights(slot_weight, aggregators, scaler_degree, csr.n_edges, dev)
     if degree_col is not None:
         d.degree_col = _check_degree_col(degree_col, csr.n_edges, dev).data_ptr()
     if view is None and row_ids is None and _dynamic_tail(csr):
@@ -200,9 +233,13 @@ def aggregate_forward(gathered: torch.Tensor, csr: CSRGraph, aggregators: Names,
         if ptr_table.dtype != torch.int64 or ptr_table.device != dev:
             raise ValueError("peer pointer table must be an int64 tensor on the same device")
         d.peer_gathered, d.peer_shift = ptr_table.data_ptr(), int(shift)
-    capture.pin(csr, view, scaler_degree, degree_col)
+    capture.pin(csr, view, scaler_degree, degree_col, slot_weight)
     with torch.cuda.device(dev):
-        _lib.check(_lib.lib().pna_aggregate_fwd(C.byref(d), torch.cuda.current_stream(dev).cuda_stream))
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        if weights is None:
+            _lib.check(_lib.lib().pna_aggregate_fwd(C.byref(d), stream))
+        else:
+            _lib.check(_lib.lib().pna_aggregate_fwd_weighted(C.byref(d), *weights, stream))
     return out
 
 
@@ -233,13 +270,13 @@ def aggregate_backward(grad_out: torch.Tensor, gathered: torch.Tensor, csr: CSRG
                        avg_deg: Mapping[str, float], *, towers: int = 1, row_bias: Optional[torch.Tensor] = None,
                        has_self: bool = False, messages_in_csr_order: bool = False, need_bias_grad: bool = False,
                        relu_var: bool = False, scaler_degree: Optional[torch.Tensor] = None,
-                       degree_col: Optional[torch.Tensor] = None):
+                       degree_col: Optional[torch.Tensor] = None, slot_weight: Optional[torch.Tensor] = None):
     """Gradient of the aggregation w.r.t. ``gathered`` (and ``row_bias``) through ``pna_aggregate_bwd`` (fp32 results)."""
     dev = gathered.device
     gathered = _rows2d(gathered, "gathered")
     F = int(gathered.size(1))
     N = csr.n_nodes
-    capture.pin(csr, scaler_degree, degree_col)
+    capture.pin(csr, scaler_degree, degree_col, slot_weight)
     n_aggr, aggr_codes = _lib.pack_codes(aggregators, _lib.ALL_AGGR_CODES, "aggregator")
     n_scal, scal_codes = _lib.pack_codes(scalers, _lib.SCALER_CODES, "scaler")
     grad_out = _rows2d(grad_out.to(gathered.dtype), "grad_out")
@@ -264,7 +301,8 @@ def aggregate_backward(grad_out: torch.Tensor, gathered: torch.Tensor, csr: CSRG
         hub_info=_ptr(csr.hub_info) if csr.n_hubs else None, chunk_items=_ptr(csr.chunk_items) if csr.n_hubs else None,
         n_hubs=csr.n_hubs, n_chunks=csr.n_chunks)
     if scaler_degree is not None:
-        d.scaler_degree = _check_scaler_degree(scaler_degree, N, dev).data_ptr()
+        _set_scaler_degree(d, scaler_degree, N, dev)
+    weights = _weights(slot_weight, aggregators, scaler_degree, csr.n_edges, dev)
     if degree_col is not None:
         d.degree_col = _check_degree_col(degree_col, csr.n_edges, dev).data_ptr()
     scratch = None
@@ -273,15 +311,20 @@ def aggregate_backward(grad_out: torch.Tensor, gathered: torch.Tensor, csr: CSRG
         d.hub_partials = scratch.data_ptr()
     ld_go = grad_out.stride(0) if N > 1 else grad_out.size(1)
     if deterministic:
-        _backward_deterministic(d, grad_out, ld_go, gathered, csr, gg, gb, messages_in_csr_order)
+        _backward_deterministic(d, grad_out, ld_go, gathered, csr, gg, gb, messages_in_csr_order, weights)
         return gg, gb
-    # moments and the weighted sums have no coefficient form (their per-slot gradient is not c0 + c1 * m): atomic path
+    # moments, the weighted sums and slot weights have no coefficient form (their per-slot gradient is not c0 + c1 * m):
+    # atomic path
     if messages_in_csr_order or csr.n_edges == 0 or csr.sources_unique or backward_mode() == "atomic" \
             or any(a in _lib.MOMENTS + _lib.WEIGHTED for a in _names(aggregators)) \
+            or weights is not None \
             or 2 * _round_up(F, 4) > _lib.query(_lib.QUERY_MAX_FEATURES):
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().pna_aggregate_bwd(C.byref(d), grad_out.data_ptr(), ld_go, gg.data_ptr(), F, _ptr(gb), F,
-                                                    torch.cuda.current_stream(dev).cuda_stream))
+            args = (grad_out.data_ptr(), ld_go, gg.data_ptr(), F, _ptr(gb), F, torch.cuda.current_stream(dev).cuda_stream)
+            if weights is None:
+                _lib.check(_lib.lib().pna_aggregate_bwd(C.byref(d), *args))
+            else:
+                _lib.check(_lib.lib().pna_aggregate_bwd_weighted(C.byref(d), *weights, *args))
         return gg, gb
     # shared source rows: coefficients per destination row -> their sums over the out-edges of every source row (the
     # forward kernels on the transposed graph) -> grad_gathered; the only atomics route min / max (one per row and feature)
@@ -317,7 +360,8 @@ def deterministic_slab_width(n_edges: int, n_feat: int, align: int) -> int:
     return max(align, min(w, max_f))
 
 
-def _backward_deterministic(d, grad_out, ld_go, gathered, csr: CSRGraph, gg, gb, messages_in_csr_order: bool) -> None:
+def _backward_deterministic(d, grad_out, ld_go, gathered, csr: CSRGraph, gg, gb, messages_in_csr_order: bool,
+                            weights=None) -> None:
     """No floating-point atomics: per feature slab, (1) ``pna_aggregate_bwd_slots`` stores the gradient of every message in
     CSR slot order, (2) the forward kernel sums those rows over the slot-transposed CSR (ascending slot ids per source row)
     into the ``gg`` column slab.  Messages in CSR order need step 1 only: its output is their gradient."""
@@ -325,10 +369,15 @@ def _backward_deterministic(d, grad_out, ld_go, gathered, csr: CSRGraph, gg, gb,
     F, E = gg.size(1), csr.n_edges
     L = _lib.lib()
     stream = torch.cuda.current_stream(dev).cuda_stream
+
+    def slots(*args):          # pna_aggregate_bwd_slots, or its weighted form (slot_weight, scaler_degree_f)
+        if weights is None:
+            return L.pna_aggregate_bwd_slots(C.byref(d), *args)
+        return L.pna_aggregate_bwd_slots_weighted(C.byref(d), *weights, *args)
     if messages_in_csr_order:
         gs = gg if E else torch.empty((1, F), dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(L.pna_aggregate_bwd_slots(C.byref(d), grad_out.data_ptr(), ld_go, 0, F, gs.data_ptr(), F, _ptr(gb), F, stream))
+            _lib.check(slots(grad_out.data_ptr(), ld_go, 0, F, gs.data_ptr(), F, _ptr(gb), F, stream))
         return
     w = deterministic_slab_width(E, F, 16 // gathered.element_size())
     buf = torch.empty(max(E, 1) * w, dtype=torch.float32, device=dev)
@@ -337,8 +386,7 @@ def _backward_deterministic(d, grad_out, ld_go, gathered, csr: CSRGraph, gg, gb,
         fc = min(w, F - f0)
         gs = buf[:max(E, 1) * fc].view(max(E, 1), fc)
         with torch.cuda.device(dev):
-            _lib.check(L.pna_aggregate_bwd_slots(C.byref(d), grad_out.data_ptr(), ld_go, f0, fc, gs.data_ptr(), fc, _ptr(gb), F,
-                                                 stream))
+            _lib.check(slots(grad_out.data_ptr(), ld_go, f0, fc, gs.data_ptr(), fc, _ptr(gb), F, stream))
         if E:
             aggregate_forward(gs, tcsr, ["sum"], ["identity"], {"log": 1.0, "lin": 1.0}, out=gg[:, f0:f0 + fc])
 
@@ -362,24 +410,25 @@ def backward_mode() -> str:
 class _PNAAggregate(torch.autograd.Function):
     @staticmethod
     def forward(ctx, gathered, row_bias, self_feat, csr, aggregators, scalers, avg_deg, towers, self_divided,
-                messages_in_csr_order, zero_isolated, relu_var=False, scaler_degree=None, degree_col=None):
+                messages_in_csr_order, zero_isolated, relu_var=False, scaler_degree=None, degree_col=None, slot_weight=None):
         out = aggregate_forward(gathered, csr, aggregators, scalers, avg_deg, towers=towers, row_bias=row_bias,
                                 self_feat=self_feat, self_divided=self_divided,
                                 messages_in_csr_order=messages_in_csr_order, zero_isolated=zero_isolated, relu_var=relu_var,
-                                scaler_degree=scaler_degree, degree_col=degree_col)
+                                scaler_degree=scaler_degree, degree_col=degree_col, slot_weight=slot_weight)
         ctx.save_for_backward(gathered, row_bias, self_feat)
         ctx.meta = (csr, _names(aggregators), _names(scalers), dict(avg_deg), towers, self_divided, messages_in_csr_order,
-                    relu_var, scaler_degree, degree_col)
+                    relu_var, scaler_degree, degree_col, slot_weight)
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
         gathered, row_bias, self_feat = ctx.saved_tensors
-        csr, aggregators, scalers, avg_deg, towers, self_divided, in_order, relu_var, scaler_degree, degree_col = ctx.meta
+        csr, aggregators, scalers, avg_deg, towers, self_divided, in_order, relu_var, scaler_degree, degree_col, slot_weight = \
+            ctx.meta
         grad_g, grad_b = aggregate_backward(
             grad_out, gathered, csr, aggregators, scalers, avg_deg, towers=towers, row_bias=row_bias,
             has_self=self_feat is not None, messages_in_csr_order=in_order, need_bias_grad=ctx.needs_input_grad[1],
-            relu_var=relu_var, scaler_degree=scaler_degree, degree_col=degree_col)
+            relu_var=relu_var, scaler_degree=scaler_degree, degree_col=degree_col, slot_weight=slot_weight)
         gs = None
         if self_feat is not None and ctx.needs_input_grad[2]:
             # the self block of every tower is a plain copy: its gradient is the matching slice of grad_out
@@ -389,24 +438,28 @@ class _PNAAggregate(torch.autograd.Function):
             gs = (blk.reshape(N, F) if self_divided else blk.sum(1)).to(self_feat.dtype)
         return (grad_g.to(gathered.dtype) if ctx.needs_input_grad[0] else None,
                 grad_b.to(row_bias.dtype) if (grad_b is not None) else None, gs,
-                None, None, None, None, None, None, None, None, None, None, None)
+                None, None, None, None, None, None, None, None, None, None, None, None)
 
 
 def pna_aggregate(gathered: torch.Tensor, csr: CSRGraph, aggregators: Names, scalers: Names,
                   avg_deg: Mapping[str, float], *, towers: int = 1, row_bias: Optional[torch.Tensor] = None,
                   self_feat: Optional[torch.Tensor] = None, self_divided: bool = True,
                   messages_in_csr_order: bool = False, zero_isolated: bool = False, relu_var: bool = False,
-                  scaler_degree: Optional[torch.Tensor] = None, degree_col: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """Differentiable PNA aggregation (forward = one libpna_sm90 call).  See :func:`aggregate_forward`."""
+                  scaler_degree: Optional[torch.Tensor] = None, degree_col: Optional[torch.Tensor] = None,
+                  slot_weight: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Differentiable PNA aggregation (forward = one libpna_sm90 call).  See :func:`aggregate_forward`.  ``slot_weight`` is a
+    constant: a tensor that requires grad is refused (no gradient flows to it)."""
+    if slot_weight is not None and slot_weight.requires_grad and torch.is_grad_enabled():
+        raise ValueError("slot_weight gets no gradient: pass a tensor that does not require grad (e.g. weight.detach())")
     needs_grad = torch.is_grad_enabled() and any(
         t is not None and t.requires_grad for t in (gathered, row_bias, self_feat))
     if not needs_grad:
         return aggregate_forward(gathered, csr, aggregators, scalers, avg_deg, towers=towers, row_bias=row_bias,
                                  self_feat=self_feat, self_divided=self_divided,
                                  messages_in_csr_order=messages_in_csr_order, zero_isolated=zero_isolated, relu_var=relu_var,
-                                 scaler_degree=scaler_degree, degree_col=degree_col)
+                                 scaler_degree=scaler_degree, degree_col=degree_col, slot_weight=slot_weight)
     return _PNAAggregate.apply(gathered, row_bias, self_feat, csr, aggregators, scalers, avg_deg, towers, self_divided,
-                               messages_in_csr_order, zero_isolated, relu_var, scaler_degree, degree_col)
+                               messages_in_csr_order, zero_isolated, relu_var, scaler_degree, degree_col, slot_weight)
 
 
 def avg_deg_from_histogram(deg: torch.Tensor) -> dict:

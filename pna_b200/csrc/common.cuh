@@ -66,9 +66,7 @@ struct DegScales {
     }
   }
 };
-__device__ __forceinline__ DegScales deg_scales(int deg, float avg_log, float avg_lin) {
-  const bool iso = deg == 0;
-  const float degf = (float)deg;
+__device__ __forceinline__ DegScales deg_scales_of(bool iso, float degf, float avg_log, float avg_lin) {
   const float lg = logf(degf + 1.0f);
   DegScales s;
   s.amp = __fdiv_rn(lg, avg_log);                      // scalers.py:12-13  (0 for an isolated row)
@@ -76,6 +74,13 @@ __device__ __forceinline__ DegScales deg_scales(int deg, float avg_log, float av
   s.lin = __fdiv_rn(degf, avg_lin);                    // scalers.py:22-23
   s.ilin = iso ? 1.0f : __fdiv_rn(avg_lin, degf);      // scalers.py:26-29
   return s;
+}
+__device__ __forceinline__ DegScales deg_scales(int deg, float avg_log, float avg_lin) {
+  return deg_scales_of(deg == 0, (float)deg, avg_log, avg_lin);
+}
+// a real-valued degree (scaler_degree_f of pna_aggregate_fwd_weighted: D = adj.sum(-1) of a weighted dense adjacency)
+__device__ __forceinline__ DegScales deg_scales_f(float deg, float avg_log, float avg_lin) {
+  return deg_scales_of(deg == 0.0f, deg, avg_log, avg_lin);
 }
 
 // ---- element load/store with fp32 math -------------------------------------------------------------------

@@ -78,11 +78,34 @@ static int launch_addons_fwd(const pna_agg_t* d, cudaStream_t st) {
   return PNA_OK;
 }
 
+// A weighted call (pna_aggregate_fwd_weighted): every column, in place of the existing kernels.
+template <typename T>
+static int launch_adj_weight_fwd(const AWParams& a, cudaStream_t st) {
+  const MParams& p = a.m;
+  const unsigned gy = (unsigned)((p.F + 31) / 32);
+  constexpr long long per_block = kMomThreads / 32;
+  if (!(p.flags & PNA_FLAG_SKIP_LIGHT)) {
+    const long long gx = (p.n_rows + per_block - 1) / per_block;
+    PNA_REQUIRE(gx <= 0x7fffffffll, PNA_ERR_UNSUPPORTED, "pna_aggregate_fwd: too many rows");
+    k_aw_rows<T><<<dim3((unsigned)gx, gy), kMomThreads, 0, st>>>(a);
+    PNA_CUDA_TRY(cudaGetLastError());
+  }
+  if (!(p.flags & PNA_FLAG_SKIP_HUBS) && p.n_hubs > 0) {
+    const unsigned gc = (unsigned)((p.n_chunks + per_block - 1) / per_block), gh = (unsigned)((p.n_hubs + per_block - 1) / per_block);
+    k_aw_chunk<T><<<dim3(gc, gy), kMomThreads, 0, st>>>(a);
+    PNA_CUDA_TRY(cudaGetLastError());
+    k_aw_hub_final<T><<<dim3(gh, gy), kMomThreads, 0, st>>>(a);
+    PNA_CUDA_TRY(cudaGetLastError());
+  }
+  return PNA_OK;
+}
+
 }  // namespace pna
 
 using namespace pna;
 
-extern "C" int pna_aggregate_fwd(const pna_agg_t* d, pna_stream_t stream) {
+// sw / sdf: pna_aggregate_fwd_weighted's slot weights and real-valued scaler degree (both NULL: pna_aggregate_fwd)
+static int fwd_entry(const pna_agg_t* d, const float* sw, const float* sdf, pna_stream_t stream) {
   PNA_REQUIRE(d != nullptr, PNA_ERR_BAD_ARG, "pna_aggregate_fwd: null descriptor");
   PNA_REQUIRE(d->n_rows >= 0 && d->n_feat > 0 && d->n_towers > 0, PNA_ERR_BAD_ARG,
               "pna_aggregate_fwd: bad sizes n_rows=%lld n_feat=%d n_towers=%d", (long long)d->n_rows, d->n_feat,
@@ -109,12 +132,27 @@ extern "C" int pna_aggregate_fwd(const pna_agg_t* d, pna_stream_t stream) {
   PNA_REQUIRE(d->dtype == PNA_F32 || d->dtype == PNA_BF16, PNA_ERR_UNSUPPORTED, "pna_aggregate_fwd: dtype %d", d->dtype);
   PNA_REQUIRE(!((weighted >> (PNA_AGGR_NORMALISED_MEAN - PNA_AGGR_SOFTMAX)) & 1u) || d->col || d->degree_col,
               PNA_ERR_UNSUPPORTED, "pna_aggregate_fwd: normalised_mean needs col or degree_col (the source of every slot)");
+  const bool adj_weight = sw || sdf;
+  if (adj_weight) {
+    for (int a = 0; a < d->n_aggr; ++a)
+      PNA_REQUIRE(adj_weight_code((d->aggr_codes >> (4 * a)) & 15u), PNA_ERR_UNSUPPORTED,
+                  "pna_aggregate_fwd: slot_weight / scaler_degree_f take sum, mean, min, max, var and std only");
+    PNA_REQUIRE(!d->peer_gathered && !d->row_ids, PNA_ERR_UNSUPPORTED,
+                "pna_aggregate_fwd: slot_weight / scaler_degree_f are not available with peer_gathered or row_ids");
+  }
   if (d->n_rows == 0) return PNA_OK;
   PNA_REQUIRE(d->gathered && d->rowptr && d->out, PNA_ERR_BAD_ARG, "pna_aggregate_fwd: null gathered/rowptr/out");
   PNA_REQUIRE(d->split_threshold >= 2 && d->chunk_edges >= 1, PNA_ERR_BAD_ARG, "pna_aggregate_fwd: bad split/chunk");
   if (d->n_hubs > 0 && !(d->flags & PNA_FLAG_SKIP_HUBS))
     PNA_REQUIRE(d->hub_info && d->chunk_items && d->hub_partials, PNA_ERR_BAD_ARG,
                 "pna_aggregate_fwd: n_hubs=%lld but hub_info/chunk_items/hub_partials missing", (long long)d->n_hubs);
+  if (adj_weight) {
+    PNA_REQUIRE(d->ld_out >= (long long)d->n_towers * ((d->self_feat ? 1 : 0) + d->n_aggr * d->n_scalers) * (d->n_feat / d->n_towers),
+                PNA_ERR_BAD_ARG, "pna_aggregate_fwd: ld_out smaller than the row width");
+    const AWParams a = adj_weight_params(d, sw, sdf);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    return d->dtype == PNA_F32 ? launch_adj_weight_fwd<float>(a, st) : launch_adj_weight_fwd<__nv_bfloat16>(a, st);
+  }
 
   KParams p;
   p.x = d->gathered; p.ldx = d->ld_gathered;
@@ -170,4 +208,11 @@ extern "C" int pna_aggregate_fwd(const pna_agg_t* d, pna_stream_t stream) {
   }
   if (rc != PNA_OK || !addons) return rc;
   return d->dtype == PNA_F32 ? launch_addons_fwd<float>(d, st) : launch_addons_fwd<__nv_bfloat16>(d, st);
+}
+
+extern "C" int pna_aggregate_fwd(const pna_agg_t* d, pna_stream_t stream) { return fwd_entry(d, nullptr, nullptr, stream); }
+
+extern "C" int pna_aggregate_fwd_weighted(const pna_agg_t* d, const float* slot_weight, const float* scaler_degree_f,
+                                          pna_stream_t stream) {
+  return fwd_entry(d, slot_weight, scaler_degree_f, stream);
 }

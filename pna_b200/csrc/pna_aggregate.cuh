@@ -389,3 +389,4 @@ __device__ __forceinline__ void finalize_row_ds(const KParams& p, const FeatMap<
 
 #include "pna_aggregate_moments.cuh"
 #include "pna_aggregate_weighted.cuh"
+#include "pna_aggregate_adj_weight.cuh"

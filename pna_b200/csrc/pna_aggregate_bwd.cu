@@ -97,15 +97,12 @@ __device__ __forceinline__ void load_m(const KParams& p, int src, int f, const f
   }
 }
 
-// upstream gradients of one row -> the two coefficients and the min / max gradients
+// upstream gradients of one row -> the two coefficients and the min / max gradients.  cnt: what the row's moments divide by
+// (the slot count, clamped at 1; W_i for slot weights); sdegf: the scalers' degree, siso = (it is 0).
 template <typename T, int VEC>
-__device__ __forceinline__ void coefficients(const BParams& b, long long row, int deg, int ooff, const Stats<VEC>& st, Coef<VEC>& c) {
+__device__ __forceinline__ void coefficients_at(const BParams& b, long long row, float cnt, bool siso, float sdegf, int ooff,
+                                                const Stats<VEC>& st, Coef<VEC>& c) {
   const KParams& p = b.k;
-  const bool iso = deg == 0;
-  const float degf = (float)deg, cnt = iso ? 1.0f : degf;
-  const int sdeg = p.sdeg ? __ldg(p.sdeg + row) : deg;      // degree seen by the scalers (pna_agg_t.scaler_degree)
-  const bool siso = sdeg == 0;
-  const float sdegf = (float)sdeg;
   const float lg = logf(sdegf + 1.0f);
   const float s_amp = lg / p.avg_log, s_att = siso ? 1.0f : p.avg_log / lg;
   const float s_lin = sdegf / p.avg_lin, s_ilin = siso ? 1.0f : p.avg_lin / sdegf;
@@ -149,6 +146,15 @@ __device__ __forceinline__ void coefficients(const BParams& b, long long row, in
       }
     }
   }
+}
+
+template <typename T, int VEC>
+__device__ __forceinline__ void coefficients(const BParams& b, long long row, int deg, int ooff, const Stats<VEC>& st, Coef<VEC>& c) {
+  const KParams& p = b.k;
+  const bool iso = deg == 0;
+  const float degf = (float)deg, cnt = iso ? 1.0f : degf;
+  const int sdeg = p.sdeg ? __ldg(p.sdeg + row) : deg;      // degree seen by the scalers (pna_agg_t.scaler_degree)
+  coefficients_at<T, VEC>(b, row, cnt, sdeg == 0, (float)sdeg, ooff, st, c);
 }
 
 template <int VEC>
@@ -679,6 +685,172 @@ static int launch_addons_bwd(const pna_agg_t* d, const MParams& mp, cudaStream_t
   return PNA_OK;
 }
 
+// ---- slot weights (pna_aggregate_bwd_weighted / _bwd_slots_weighted; forward and formulas: pna_aggregate_adj_weight.cuh) --
+// The gradient of slot s is  g_s = fl(w_s * fl(c0 + c1 * m_s)) + [s == argmin] gmin + [s == argmax] gmax,  with c0, c1, gmin,
+// gmax from coefficients_at at cnt = W_i (and the scalers at D), the statistics S, Q of the weighted forward and min / max
+// over the positive-weight slots (first slot attaining them); message_grad evaluates both steps, so all-ones weights give
+// the unweighted per-slot bits.  One thread per (row or chunk, feature column) as in the forward; split rows:
+// (1) per chunk S, Q, min, max, arg slots into [0..5]; (2) per split row their chunk-order merge -> the coefficients into
+// the row's slot (n_chunks + h) [0..5]; (3) per chunk the slot gradients and the chunk's slot-order share of grad_row_bias
+// into [0]; (4) per split row those shares added in chunk order.  SLOTS stores g_s into grad_slots; the atomic instance
+// adds it into grad_gathered[col[s]] (per-slot rows, col == NULL: stores).  grad_row_bias is stored, never accumulated.
+struct AWBParams {
+  AWParams a;
+  BParams b;
+};
+
+__device__ __forceinline__ float aw_slot_grad(const Coef<1>& c, float w, float m, bool is_min, bool is_max) {
+  return message_grad(0.f, w, message_grad(c.c0[0], c.c1[0], m, false, 0.f, false, 0.f), is_min, c.gmin[0], is_max, c.gmax[0]);
+}
+
+// statistics of slots [beg, end) in the layout of the unweighted backward (Stats<1>: S, Q, min, max and their first slot)
+template <typename T>
+__device__ __forceinline__ Stats<1> aw_stats(const AWParams& a, int beg, int end, int f, float b, bool hb) {
+  Stats<1> st;
+  st.init();
+  for (int e = beg; e < end; ++e) {
+    const float m = mom_msg<T>(a.m, e, f, b, hb), ws = aw_weight(a.w, e);
+    st.sum[0] = __fadd_rn(st.sum[0], __fmul_rn(m, ws));
+    st.sq[0] = __fadd_rn(st.sq[0], __fmul_rn(__fmul_rn(m, m), ws));
+    if (ws > 0.f) {
+      if (m < st.mn[0]) { st.mn[0] = m; st.amn[0] = e; }
+      if (m > st.mx[0]) { st.mx[0] = m; st.amx[0] = e; }
+    }
+  }
+  return st;
+}
+
+template <typename T>
+__device__ __forceinline__ void aw_coef(const AWBParams& q, long long row, int beg, int deg, int f, const Stats<1>& st, Coef<1>& c) {
+  const MParams& p = q.a.m;
+  const float D = aw_scaler_degree(p, q.a.sdf, row, deg);
+  coefficients_at<T, 1>(q.b, row, aw_weight_sum(q.a.w, beg, beg + deg), D == 0.0f, D, (int)mom_base_col(p, f), st, c);
+}
+
+// add every slot's gradient of [beg, end) to its destination; returns their slot-order sum
+template <typename T, bool SLOTS>
+__device__ __forceinline__ float aw_emit(const AWParams& a, int beg, int end, int f, float b, bool hb, const Coef<1>& c, int amn,
+                                         int amx) {
+  const MParams& p = a.m;
+  float acc = 0.f;
+  for (int e = beg; e < end; ++e) {
+    const float g = aw_slot_grad(c, aw_weight(a.w, e), mom_msg<T>(p, e, f, b, hb), e == amn, e == amx);
+    acc = __fadd_rn(acc, g);
+    if constexpr (SLOTS) {
+      p.gs[(long long)e * p.ldgs + (f - p.f0)] = g;
+    } else {
+      if (p.col) atomicAdd(p.gg + (long long)__ldg(p.col + e) * p.ldgg + f, g);
+      else p.gg[(long long)e * p.ldgg + f] = g;
+    }
+  }
+  return acc;
+}
+
+template <typename T, bool SLOTS>
+__global__ void __launch_bounds__(kMomThreads) k_aw_bwd_rows(const AWBParams q) {
+  const MParams& p = q.a.m;
+  long long row; int f;
+  if (!mom_thread(p, p.n_rows, row, f)) return;
+  const int beg = __ldg(p.rowptr + row), end = __ldg(p.rowptr + row + 1), deg = end - beg;
+  if (deg >= p.split) return;
+  float gbs = 0.f;
+  if (deg > 0) {
+    const bool hb = p.bias != nullptr;
+    const float b = mom_bias<T>(p, row, f);
+    const Stats<1> st = aw_stats<T>(q.a, beg, end, f, b, hb);
+    Coef<1> c;
+    aw_coef<T>(q, row, beg, deg, f, st, c);
+    gbs = aw_emit<T, SLOTS>(q.a, beg, end, f, b, hb, c, st.amn[0], st.amx[0]);
+  }
+  if (p.gb) p.gb[row * p.ldgb + f] = gbs;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kMomThreads) k_aw_bwd_chunk_stats(const AWBParams q) {
+  const MParams& p = q.a.m;
+  long long c; int f;
+  if (!mom_thread(p, p.n_chunks, c, f)) return;
+  const MomChunk m = mom_chunk(p, c);
+  const Stats<1> st = aw_stats<T>(q.a, m.beg, m.end, f, mom_bias<T>(p, m.row, f), p.bias != nullptr);
+  *mom_part<6>(p, c, 0, f) = st.sum[0]; *mom_part<6>(p, c, 1, f) = st.sq[0];
+  *mom_part<6>(p, c, 2, f) = st.mn[0]; *mom_part<6>(p, c, 3, f) = st.mx[0];
+  *mom_part<6>(p, c, 4, f) = __int_as_float(st.amn[0]); *mom_part<6>(p, c, 5, f) = __int_as_float(st.amx[0]);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kMomThreads) k_aw_bwd_hub_coef(const AWBParams q) {
+  const MParams& p = q.a.m;
+  long long h; int f;
+  if (!mom_thread(p, p.n_hubs, h, f)) return;
+  const long long row = __ldg(p.hub_info + 4 * h);
+  const int first = __ldg(p.hub_info + 4 * h + 1), nch = __ldg(p.hub_info + 4 * h + 2), deg = __ldg(p.hub_info + 4 * h + 3);
+  Stats<1> st;
+  st.init();
+  for (int j = 0; j < nch; ++j) {
+    st.sum[0] = __fadd_rn(st.sum[0], *mom_part<6>(p, first + j, 0, f));
+    st.sq[0] = __fadd_rn(st.sq[0], *mom_part<6>(p, first + j, 1, f));
+    const float mn = *mom_part<6>(p, first + j, 2, f), mx = *mom_part<6>(p, first + j, 3, f);
+    if (mn < st.mn[0]) { st.mn[0] = mn; st.amn[0] = __float_as_int(*mom_part<6>(p, first + j, 4, f)); }
+    if (mx > st.mx[0]) { st.mx[0] = mx; st.amx[0] = __float_as_int(*mom_part<6>(p, first + j, 5, f)); }
+  }
+  Coef<1> c;
+  aw_coef<T>(q, row, __ldg(p.rowptr + row), deg, f, st, c);
+  const long long hs = p.n_chunks + h;
+  *mom_part<6>(p, hs, 0, f) = c.c0[0]; *mom_part<6>(p, hs, 1, f) = c.c1[0];
+  *mom_part<6>(p, hs, 2, f) = c.gmin[0]; *mom_part<6>(p, hs, 3, f) = c.gmax[0];
+  *mom_part<6>(p, hs, 4, f) = __int_as_float(st.amn[0]); *mom_part<6>(p, hs, 5, f) = __int_as_float(st.amx[0]);
+}
+
+template <typename T, bool SLOTS>
+__global__ void __launch_bounds__(kMomThreads) k_aw_bwd_chunk_grad(const AWBParams q) {
+  const MParams& p = q.a.m;
+  long long c; int f;
+  if (!mom_thread(p, p.n_chunks, c, f)) return;
+  const MomChunk m = mom_chunk(p, c);
+  const long long hs = p.n_chunks + m.h;
+  Coef<1> cf;
+  cf.c0[0] = *mom_part<6>(p, hs, 0, f); cf.c1[0] = *mom_part<6>(p, hs, 1, f);
+  cf.gmin[0] = *mom_part<6>(p, hs, 2, f); cf.gmax[0] = *mom_part<6>(p, hs, 3, f);
+  const int amn = __float_as_int(*mom_part<6>(p, hs, 4, f)), amx = __float_as_int(*mom_part<6>(p, hs, 5, f));
+  *mom_part<6>(p, c, 0, f) = aw_emit<T, SLOTS>(q.a, m.beg, m.end, f, mom_bias<T>(p, m.row, f), p.bias != nullptr, cf, amn, amx);
+}
+
+__global__ void __launch_bounds__(kMomThreads) k_aw_bwd_hub_bias(const AWBParams q) {
+  const MParams& p = q.a.m;
+  long long h; int f;
+  if (!mom_thread(p, p.n_hubs, h, f)) return;
+  const long long row = __ldg(p.hub_info + 4 * h);
+  const int first = __ldg(p.hub_info + 4 * h + 1), nch = __ldg(p.hub_info + 4 * h + 2);
+  float acc = 0.f;
+  for (int j = 0; j < nch; ++j) acc = __fadd_rn(acc, *mom_part<6>(p, first + j, 0, f));
+  p.gb[row * p.ldgb + f] = acc;
+}
+
+template <typename T, bool SLOTS>
+static int launch_adj_weight_bwd(const AWBParams& q, cudaStream_t st) {
+  const MParams& p = q.a.m;
+  const unsigned gy = (unsigned)((p.f1 - p.f0 + 31) / 32);
+  constexpr long long per_block = kMomThreads / 32;
+  const long long gx = (p.n_rows + per_block - 1) / per_block;
+  PNA_REQUIRE(gx <= 0x7fffffffll, PNA_ERR_UNSUPPORTED, "pna_aggregate_bwd: too many rows");
+  k_aw_bwd_rows<T, SLOTS><<<dim3((unsigned)gx, gy), kMomThreads, 0, st>>>(q);
+  PNA_CUDA_TRY(cudaGetLastError());
+  if (p.n_hubs > 0) {
+    const unsigned gc = (unsigned)((p.n_chunks + per_block - 1) / per_block), gh = (unsigned)((p.n_hubs + per_block - 1) / per_block);
+    k_aw_bwd_chunk_stats<T><<<dim3(gc, gy), kMomThreads, 0, st>>>(q);
+    PNA_CUDA_TRY(cudaGetLastError());
+    k_aw_bwd_hub_coef<T><<<dim3(gh, gy), kMomThreads, 0, st>>>(q);
+    PNA_CUDA_TRY(cudaGetLastError());
+    k_aw_bwd_chunk_grad<T, SLOTS><<<dim3(gc, gy), kMomThreads, 0, st>>>(q);
+    PNA_CUDA_TRY(cudaGetLastError());
+    if (p.gb) {
+      k_aw_bwd_hub_bias<<<dim3(gh, gy), kMomThreads, 0, st>>>(q);
+      PNA_CUDA_TRY(cudaGetLastError());
+    }
+  }
+  return PNA_OK;
+}
+
 // ---- phase 3 of the coefficient path: grad_gathered[j] += S0[j] + gathered[j] * S1[j] ------------------------------------
 // sums[j] = [S0 | S1] (S1 at column c1): the 'sum' of the coefficient rows over the out-edges of source row j.
 template <typename T>
@@ -705,7 +877,7 @@ using namespace pna;
 static int bwd_entry(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_out, float* grad_gathered, int64_t ld_grad_gathered,
                      float* grad_row_bias, int64_t ld_grad_row_bias, float* coef, int64_t ld_coef, int32_t coef_c1,
                      pna_stream_t stream, float* grad_slots = nullptr, int64_t ld_grad_slots = 0, int32_t f_begin = 0,
-                     int32_t f_count = 0, bool peer = false) {
+                     int32_t f_count = 0, bool peer = false, const float* sw = nullptr, const float* sdf = nullptr) {
   PNA_REQUIRE(d != nullptr, PNA_ERR_BAD_ARG, "pna_aggregate_bwd: null descriptor");
   PNA_REQUIRE(d->n_rows >= 0 && d->n_feat > 0 && d->n_towers > 0 && d->n_feat % d->n_towers == 0, PNA_ERR_BAD_ARG,
               "pna_aggregate_bwd: bad sizes");
@@ -736,6 +908,15 @@ static int bwd_entry(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_o
               "pna_aggregate_bwd: softmax / softmin / normalised_mean are not available with peer_gathered or row_ids");
   PNA_REQUIRE(!((weighted >> (PNA_AGGR_NORMALISED_MEAN - PNA_AGGR_SOFTMAX)) & 1u) || d->col || d->degree_col,
               PNA_ERR_UNSUPPORTED, "pna_aggregate_bwd: normalised_mean needs col or degree_col (the source of every slot)");
+  // the *_weighted entry points (they have no coefficient or peer-memory form: coef == NULL and peer == false here)
+  const bool adj_weight = sw || sdf;
+  if (adj_weight) {
+    for (int a = 0; a < d->n_aggr; ++a)
+      PNA_REQUIRE(adj_weight_code((d->aggr_codes >> (4 * a)) & 15u), PNA_ERR_UNSUPPORTED,
+                  "pna_aggregate_bwd: slot_weight / scaler_degree_f take sum, mean, min, max, var and std only");
+    PNA_REQUIRE(!d->peer_gathered && !d->row_ids, PNA_ERR_UNSUPPORTED,
+                "pna_aggregate_bwd: slot_weight / scaler_degree_f are not available with peer_gathered or row_ids");
+  }
   if (d->n_rows == 0) return PNA_OK;
   PNA_REQUIRE(d->gathered && d->rowptr && grad_out && (slots || grad_gathered), PNA_ERR_BAD_ARG, "pna_aggregate_bwd: null pointer");
   if (peer) {
@@ -791,11 +972,26 @@ static int bwd_entry(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_o
   }
 
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool f32 = d->dtype == PNA_F32;
+  if (adj_weight) {   // every slot's gradient from the weighted kernels alone
+    AWBParams q;
+    q.a = adj_weight_params(d, sw, sdf);
+    q.b = b;
+    MParams& mp = q.a.m;
+    mp.go = grad_out; mp.ldgo = ld_grad_out;
+    mp.gb = grad_row_bias; mp.ldgb = ld_grad_row_bias;
+    if (slots) {
+      mp.gs = grad_slots; mp.ldgs = ld_grad_slots;
+      mp.f0 = f_begin; mp.f1 = f_begin + f_count;
+      return f32 ? launch_adj_weight_bwd<float, true>(q, st) : launch_adj_weight_bwd<__nv_bfloat16, true>(q, st);
+    }
+    mp.gg = grad_gathered; mp.ldgg = ld_grad_gathered;
+    return f32 ? launch_adj_weight_bwd<float, false>(q, st) : launch_adj_weight_bwd<__nv_bfloat16, false>(q, st);
+  }
   const int esz = d->dtype == PNA_F32 ? 4 : 2;
   const int vec = 16 / esz;
   bool vec_ok = (p.Ft % vec == 0) && al16(p.x) && al16(grad_out) && (p.ldx % vec == 0) && (b.ldgo % vec == 0);
   if (p.bias) vec_ok = vec_ok && al16(p.bias) && (p.ldb % vec == 0);
-  const bool f32 = d->dtype == PNA_F32;
   int rc;
   if (peer) {
     if (f32) rc = vec_ok ? launch_bwd_typed<float, 4, true, true>(b, st) : launch_bwd_typed<float, 1, true, true>(b, st);
@@ -831,6 +1027,22 @@ extern "C" int pna_aggregate_bwd_slots(const pna_agg_t* d, const void* grad_out,
   PNA_REQUIRE(grad_slots != nullptr, PNA_ERR_BAD_ARG, "pna_aggregate_bwd_slots: null grad_slots");
   return bwd_entry(d, grad_out, ld_grad_out, nullptr, 0, grad_row_bias, ld_grad_row_bias, nullptr, 0, 0, stream, grad_slots,
                    ld_grad_slots, f_begin, f_count);
+}
+
+extern "C" int pna_aggregate_bwd_weighted(const pna_agg_t* d, const float* slot_weight, const float* scaler_degree_f,
+                                          const void* grad_out, int64_t ld_grad_out, float* grad_gathered, int64_t ld_grad_gathered,
+                                          float* grad_row_bias, int64_t ld_grad_row_bias, pna_stream_t stream) {
+  return bwd_entry(d, grad_out, ld_grad_out, grad_gathered, ld_grad_gathered, grad_row_bias, ld_grad_row_bias, nullptr, 0, 0, stream,
+                   nullptr, 0, 0, 0, false, slot_weight, scaler_degree_f);
+}
+
+extern "C" int pna_aggregate_bwd_slots_weighted(const pna_agg_t* d, const float* slot_weight, const float* scaler_degree_f,
+                                                const void* grad_out, int64_t ld_grad_out, int32_t f_begin, int32_t f_count,
+                                                float* grad_slots, int64_t ld_grad_slots, float* grad_row_bias,
+                                                int64_t ld_grad_row_bias, pna_stream_t stream) {
+  PNA_REQUIRE(grad_slots != nullptr, PNA_ERR_BAD_ARG, "pna_aggregate_bwd_slots_weighted: null grad_slots");
+  return bwd_entry(d, grad_out, ld_grad_out, nullptr, 0, grad_row_bias, ld_grad_row_bias, nullptr, 0, 0, stream, grad_slots,
+                   ld_grad_slots, f_begin, f_count, false, slot_weight, scaler_degree_f);
 }
 
 extern "C" int pna_aggregate_bwd_peer_slots(const pna_agg_t* d, const void* grad_out, int64_t ld_grad_out, int32_t f_begin,

@@ -13,8 +13,13 @@ aggregators.py:39,51) while ``mean/std/sum`` reduce over dim 2, so for node v
 Two kernel calls fill one output row (PNA_AGGR_SKIP keeps the other call's column slots).
 ``self_loop=True`` aggregates over adj + I while the scalers keep the loop-free row degree (``pna_agg_t.scaler_degree``);
 ``var`` is clamped at 0 as the reference does (PNA_FLAG_RELU_VAR).
-Restrictions (documented, not silent): 0/1 adjacency (the reference's weighted sums are not reproduced), and -- unlike
-the reference, which divides by zero -- isolated nodes get PyG semantics (a moment of a row without neighbours is 0).
+A weighted adjacency (an entry other than 0 and 1, found in the same pass as the edges) is reproduced as the reference
+computes it (aggregators.py:17-84, scalers.py:8-38): mean/sum/var/std weigh every message with a[i, j] and divide by
+W_i = sum_j a[i, j]; max/min reduce over the entries a[u, v] > 0, unweighted; the scalers use the real D = adj.sum(-1)
+(pna_aggregate_fwd_weighted: slot_weight / scaler_degree_f, DESIGN section 2 "Weighted adjacency").  It takes mean, std, sum, var, max, min and
+identity (the other aggregators raise NotImplementedError), gives adj no gradient (an adj that requires grad raises), and a
+non-finite entry raises ValueError.  Unlike the reference, which divides by zero, isolated nodes get PyG semantics (a
+moment of a row without neighbours is 0; max/min without a positive entry are 0).
 Every name of the reference registry (models/pytorch/pna/aggregators.py:149-152) is taken.
 The moments reduce over dim 2 like mean/std (self first).  ``self_loop=True`` with a moment raises NotImplementedError:
 the reference's ``aggregate_moment`` adds I to adj and then calls ``aggregate_mean(..., self_loop=True)``, which adds I
@@ -54,35 +59,63 @@ from .towers import first_layer_pack, hidden_pack
 _SELF_FIRST = ("mean", "std", "sum", "var", "moment3", "moment4", "moment5", "softmax", "softmin", "normalised_mean")
 _MOMENTS = ("moment3", "moment4", "moment5")
 _NBR_FIRST = ("max", "min")
+_ADJ_WEIGHT = ("mean", "std", "sum", "var", "max", "min", "identity")     # what a weighted adjacency takes
 
 
 class DenseGraphs:
-    """Block-diagonal CSRs of a dense batch: one for adj (row i gathers j) and one for adj^T."""
+    """Block-diagonal CSRs of a dense batch: one for adj (row i gathers j) and one for adj^T.
+
+    A weighted adjacency (an entry other than 0 and 1) also keeps ``row_weight``, the fp32 weight a[b, i, j] of every slot of
+    ``row`` (a = adj, or adj + I with ``self_loop``), takes ``colwise`` over the entries a > 0 only (the reference's max/min
+    mask), and gives the scalers the fp32 degree D = adj.sum(-1).  On a 0/1 adjacency ``row_weight`` is None and the CSRs and
+    the int32 degree are what they always were."""
 
     def __init__(self, adj: torch.Tensor, self_loop: bool = False):
         capture.guard("DenseGraphs (the CSRs of a dense batch not seen before: adj.nonzero)")
+        adj = adj.detach()          # graph constants, cached by data pointer: no autograd history (adj gets no gradient)
         B, N, _ = adj.shape
         a = adj
         if self_loop:
             a = adj + torch.eye(N, device=adj.device, dtype=adj.dtype).unsqueeze(0)
+        # (a non-finite entry, an entry other than 0 and 1), copied to the host ahead of nonzero, whose synchronisation
+        # also completes the copy: the check costs no synchronisation of its own
+        flags = torch.stack([~torch.isfinite(adj).all(), ((adj != 0) & (adj != 1)).any()])
+        host = torch.empty(2, dtype=torch.bool, pin_memory=adj.is_cuda)
+        host.copy_(flags, non_blocking=True)
         b, i, j = (a != 0).nonzero(as_tuple=True)
+        nonfinite, weighted = host.tolist()
+        if nonfinite:
+            raise ValueError("dense PNALayer: the adjacency has a non-finite entry")
         off = b * N
         self.B, self.N = B, N
-        # the scalers always see D = adj.sum(-1) of the ORIGINAL adjacency (models/pytorch/pna/scalers.py:13,21,28,35): no
-        # self loop, row degree -- also for the max/min blocks, which reduce over the other axis
-        self.scaler_degree = (adj != 0).sum(-1).reshape(B * N).to(torch.int32).contiguous()
         self.row = build_csr(j + off, i + off, B * N)        # destination i, sources j with adj[i, j] != 0
-        self.colwise = build_csr(i + off, j + off, B * N)    # destination j, sources i with adj[i, j] != 0
+        self.row_weight = None
         self._pairs = None
+        if not weighted:
+            # the scalers always see D = adj.sum(-1) of the ORIGINAL adjacency (models/pytorch/pna/scalers.py:13,21,28,35):
+            # no self loop, row degree -- also for the max/min blocks, which reduce over the other axis
+            self.scaler_degree = (adj != 0).sum(-1).reshape(B * N).to(torch.int32).contiguous()
+            self.colwise = build_csr(i + off, j + off, B * N)    # destination j, sources i with adj[i, j] != 0
+            return
+        self.scaler_degree = adj.float().sum(-1).reshape(B * N).contiguous()
+        w = a[b, i, j].float()
+        self.row_weight = w[self.row.perm.long()].contiguous()
+        pos = w > 0
+        self.colwise = build_csr(i[pos] + off[pos], j[pos] + off[pos], B * N)   # destination j, sources i with a[i, j] > 0
 
     @property
     def pairs(self):
         """Destination j, sources = the slot ids of ``row`` whose edge is (i, j) (n_src = E, ascending): the max/min CSR
-        over per-edge messages in row-slot order.  Built on first use (pretrans_layers >= 2 only)."""
+        over per-edge messages in row-slot order (a weighted adjacency: the slots of positive weight).  Built on first use
+        (pretrans_layers >= 2 only)."""
         if self._pairs is None:
             E, dev = self.row.n_edges, self.row.device
-            self._pairs = build_csr(torch.arange(E, device=dev), self.row.col.long(), self.B * self.N, n_src=E)
-            self._pairs.sources_unique = True       # every slot is the source of exactly one pair
+            slots, dst = torch.arange(E, device=dev), self.row.col.long()
+            if self.row_weight is not None:
+                keep = self.row_weight > 0
+                slots, dst = slots[keep], dst[keep]
+            self._pairs = build_csr(slots, dst, self.B * self.N, n_src=E)
+            self._pairs.sources_unique = True       # every slot is the source of at most one pair
         return self._pairs
 
 
@@ -170,6 +203,13 @@ class PNALayer(nn.Module):
     def forward(self, input, adj):
         B, N, Fin = input.shape
         graphs = dense_graphs(adj, self.self_loop)
+        if graphs.row_weight is not None:
+            bad = [a for a in self.aggregators if a not in _ADJ_WEIGHT]
+            if bad:
+                raise NotImplementedError(f"dense PNALayer: a weighted (non 0/1) adjacency takes the aggregators "
+                                          f"{_ADJ_WEIGHT} only, not {bad}")
+            if adj.requires_grad and torch.is_grad_enabled():
+                raise ValueError("dense PNALayer: a weighted adjacency gets no gradient; pass adj.detach()")
         h = input.reshape(B * N, Fin)
         T = len(self.towers)
         a1 = [a if a in _SELF_FIRST else "_skip" for a in self.aggregators]
@@ -177,21 +217,22 @@ class PNALayer(nn.Module):
         nbr = any(a != "_skip" for a in a2)
         common = dict(towers=T, self_feat=h, self_divided=self.divide_input, relu_var=True,
                       scaler_degree=graphs.scaler_degree)
+        rw = dict(slot_weight=graphs.row_weight) if graphs.row_weight is not None else {}
         if not self.towers[0].pretrans.is_single_affine():
-            out, out2, x_id = self._forward_edge_mlp(h, graphs, a1, a2, nbr, common)
+            out, out2, x_id = self._forward_edge_mlp(h, graphs, a1, a2, nbr, common, rw)
         else:
             A, Bm, b = self._halves(h)
             out2, x_id = None, lambda: A + Bm + b
             if not (torch.is_grad_enabled() and (h.requires_grad or any(p.requires_grad for p in self.parameters()))):
                 # mean/std: message = W_first h_v + W_second h_u + b, neighbours u from row v of adj
-                out = aggregate_forward(Bm + b, graphs.row, a1, self.scalers, self.avg_d, row_bias=A, **common)
+                out = aggregate_forward(Bm + b, graphs.row, a1, self.scalers, self.avg_d, row_bias=A, **common, **rw)
                 # max/min: message = W_first h_u + W_second h_v + b, neighbours u from column v of adj; fills the
                 # skipped slots
                 if nbr:
                     aggregate_forward(A + b, graphs.colwise, a2, self.scalers, self.avg_d, row_bias=Bm, out=out, **common)
             else:
                 # training (multitask_benchmark/util/train.py:148): two differentiable calls, columns merged by a mask
-                out = pna_aggregate(Bm + b, graphs.row, a1, self.scalers, self.avg_d, row_bias=A, **common)
+                out = pna_aggregate(Bm + b, graphs.row, a1, self.scalers, self.avg_d, row_bias=A, **common, **rw)
                 if nbr:
                     out2 = pna_aggregate(A + b, graphs.colwise, a2, self.scalers, self.avg_d, row_bias=Bm, **common)
         if out2 is not None:
@@ -207,7 +248,7 @@ class PNALayer(nn.Module):
         y = torch.cat([tw.posttrans(out[:, t]) for t, tw in enumerate(self.towers)], dim=1)
         return self.mixing_network(y).view(B, N, -1)
 
-    def _forward_edge_mlp(self, h, graphs, a1, a2, nbr, common):
+    def _forward_edge_mlp(self, h, graphs, a1, a2, nbr, common, rw):
         """pretrans_layers >= 2: per-edge messages from pna_edge_mlp_fwd (module docstring) and their aggregation.  Returns
         the self-first aggregate, the neighbour-first one (None without max/min) and a callable giving the identity
         block's pretrans([h_i, h_i]); ``forward`` merges them as on the affine path."""
@@ -219,7 +260,7 @@ class PNALayer(nn.Module):
         # self first: row i reads the messages of its own slots; normalised_mean weighs slot s with D of col[s]
         dcol = graphs.row.col if "normalised_mean" in self.aggregators else None
         out = pna_aggregate(M, graphs.row, a1, self.scalers, self.avg_d, messages_in_csr_order=True, degree_col=dcol,
-                            **common)
+                            **common, **rw)
         # neighbour first: node v reduces X[u, v] = M[slot of edge (u, v)] over u
         out2 = pna_aggregate(M, graphs.pairs, a2, self.scalers, self.avg_d, **common) if nbr else None
         it = self.input_tower
@@ -228,15 +269,18 @@ class PNALayer(nn.Module):
 
     def _identity_block(self, x_id, graphs):
         """[B*N, T * (1 + S*A) * F_t]: x_id's tower slice times each scaler's factor in every (scaler, aggregator) slot; the
-        factors are the aggregation epilogue's (common.cuh deg_scales: attenuation / inverse_linear are 1 where D == 0)."""
+        factors are the aggregation epilogue's (common.cuh deg_scales: attenuation / inverse_linear are 1 where D == 0);
+        D is the int32 row degree, or the fp32 adj.sum(-1) of a weighted adjacency."""
         T, Ft = len(self.towers), self.input_tower
         A, S = len(self.aggregators), len(self.scalers)
         D = graphs.scaler_degree.to(x_id.dtype)
         lg = torch.log(D + 1)
         one = torch.ones_like(D)
         avg_log, avg_lin = self.avg_d["log"], self.avg_d.get("lin", 1.0)
-        fac = {"identity": one, "amplification": lg / avg_log, "attenuation": torch.where(D > 0, avg_log / lg, one),
-               "linear": D / avg_lin, "inverse_linear": torch.where(D > 0, avg_lin / D, one)}
+        # D != 0, not D > 0: a signed adjacency can have a row sum in (-1, 0), where the reference and the kernels' deg_scales_f
+        # divide as usual
+        fac = {"identity": one, "amplification": lg / avg_log, "attenuation": torch.where(D != 0, avg_log / lg, one),
+               "linear": D / avg_lin, "inverse_linear": torch.where(D != 0, avg_lin / D, one)}
         f = torch.stack([fac[s_] for s_ in self.scalers], 1)                         # [B*N, S]
         v = x_id.view(-1, T, 1, 1, Ft) * f.view(-1, 1, S, 1, 1)                      # [B*N, T, S, 1, F_t]
         v = v.expand(-1, T, S, A, Ft).reshape(-1, T, S * A, Ft)
