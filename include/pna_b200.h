@@ -168,6 +168,31 @@ int pna_csr_light_view(const int32_t* rowptr, const int32_t* col, int64_t n_node
                        void* workspace, size_t workspace_bytes, pna_stream_t stream);
 int pna_csr_light_view_workspace_bytes(int64_t n_nodes, size_t* bytes);
 
+/* Bytes of device scratch pna_csr_build_padded needs for the capacities (n_nodes, n_edges). */
+int pna_csr_padded_workspace_bytes(int64_t n_nodes, int64_t n_edges, size_t* bytes);
+
+/* CSR of a padded edge list into fixed capacities, with nothing read back: legal on a stream that is capturing a CUDA
+ * graph (kernel launches, CUB sort / scan in the workspace and cudaMemsetAsync only; no synchronisation).
+ *   src / dst: int64 device arrays of csr->n_edges = E entries (the edge capacity); csr->n_nodes = N is the row capacity.
+ *   An edge with dst == -1 is padding.  Any other endpoint outside dst [0, N) / src [0, n_src) sets bit 0 of status[0]
+ *   and the edge is dropped like padding (never read past the check).
+ *   Output: the row CSR of the real edges, by the stable radix sort of pna_csr_build keyed on dst (padding keyed to the
+ *   sentinel N).  rowptr[N] = number of real edges; slots rowptr[N] .. E-1 are padding with col = 0 and perm = their
+ *   original edge id.  The light view (optional, as for pna_csr_build) covers the N rows with its part partition.
+ *   split_threshold must exceed n_edges (else PNA_ERR_BAD_ARG): no row is split, every row is reduced by the light-row
+ *   kernels in slot order.  n_hubs = n_chunks = max_degree = n_light_edges = 0 and hot_source_fraction = 0 on return; cap_hubs,
+ *   cap_chunks, hub_info and chunk_items are not read.
+ *   status: int32[4] on the device, written by the stream: error bits, real edges, max in-degree, reserved.
+ *   workspace: pna_csr_padded_workspace_bytes(N, E) bytes, 256-byte aligned. */
+int pna_csr_build_padded(const int64_t* src, const int64_t* dst, pna_csr_t* csr, int32_t* status, void* workspace,
+                         size_t workspace_bytes, pna_stream_t stream);
+
+/* Per-slot arrays of a (padded) CSR with n_rows rows and n_slots slots, one kernel: for a real slot s < rowptr[n_rows],
+ * transpose_dst[s] = col[s] (the destination key of the slot-transposed build) and dst_of_slot[s] = the row owning s; for a
+ * padding slot -1 and 0.  int64 device arrays of n_slots entries.  Capture-legal. */
+int pna_csr_slot_rows(const int32_t* rowptr, const int32_t* col, int64_t n_rows, int64_t n_slots, int64_t* transpose_dst,
+                      int64_t* dst_of_slot, pna_stream_t stream);
+
 /* ---- the aggregation ("single hand-written sm_90a CUDA kernel", north_star) ------------------------------
  * For every destination row i (PyG semantics; In(i) = slots rowptr[i]..rowptr[i+1], d = |In(i)|):
  *   m_s   = gathered[col[s]] (+ row_bias[i] when given)          s in In(i)           pna.py:137-150 / :239-240

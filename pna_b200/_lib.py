@@ -32,6 +32,7 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-
 # status codes / enums of include/pna_b200.h
 ABI_VERSION = 8
 PNA_OK = 0
+PNA_ERR_INDEX = -4         # an edge endpoint outside its range (pna_csr_build; the status word of pna_csr_build_padded)
 PNA_ERR_CAPTURING = -6     # pna_csr_build / pna_csr_light_view on a stream that is capturing a CUDA graph
 PNA_F32, PNA_BF16 = 0, 1
 AGGR_CODES = {"sum": 0, "mean": 1, "min": 2, "max": 3, "var": 4, "std": 5, "_skip": 15}
@@ -55,7 +56,7 @@ EXPORTED_SYMBOLS = ("pna_csr_workspace_bytes", "pna_csr_build", "pna_csr_light_v
                     "pna_edge_mlp_bwd", "pna_edge_msg_fwd", "pna_edge_msg_bwd", "pna_query", "pna_last_error",
                     "pna_linear_towers_scaled_fwd", "pna_linear_towers_bwd_data", "pna_edge_msg_fwd_bf16", "pna_edge_msg_bwd_bf16",
                     "pna_linear_towers_scaled_fwd_bf16", "pna_aggregate_fwd_weighted", "pna_aggregate_bwd_weighted",
-                    "pna_aggregate_bwd_slots_weighted")
+                    "pna_aggregate_bwd_slots_weighted", "pna_csr_padded_workspace_bytes", "pna_csr_build_padded", "pna_csr_slot_rows")
 
 
 class PnaError(RuntimeError):
@@ -166,6 +167,12 @@ def lib() -> C.CDLL:
         L.pna_csr_workspace_bytes.argtypes = [C.c_int64, C.c_int64, C.POINTER(C.c_size_t)]
         L.pna_csr_build.restype = C.c_int
         L.pna_csr_build.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(CsrStruct), C.c_void_p, C.c_size_t, C.c_void_p]
+        L.pna_csr_padded_workspace_bytes.restype = C.c_int
+        L.pna_csr_padded_workspace_bytes.argtypes = [C.c_int64, C.c_int64, C.POINTER(C.c_size_t)]
+        L.pna_csr_build_padded.restype = C.c_int
+        L.pna_csr_build_padded.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(CsrStruct), C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+        L.pna_csr_slot_rows.restype = C.c_int
+        L.pna_csr_slot_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
         L.pna_csr_light_view.restype = C.c_int
         L.pna_csr_light_view.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]

@@ -37,6 +37,12 @@ def _rows2d(t: torch.Tensor, what: str) -> torch.Tensor:
     return t
 
 
+def _padded(csr) -> bool:
+    """Was ``csr`` built into fixed capacities (``CSRGraph.padded``)?  The aggregation takes any object with the CSR fields
+    it reads, so one without the field is an ordinary CSR."""
+    return getattr(csr, "padded", False)
+
+
 HOT_SOURCE_FRACTION_FOR_L1 = 0.25      # CSRGraph.hot_source_fraction above which the gathers also allocate in L1
 
 
@@ -245,10 +251,11 @@ def aggregate_forward(gathered: torch.Tensor, csr: CSRGraph, aggregators: Names,
 
 def row_scales(csr: CSRGraph, scalers: Names, avg_deg: Mapping[str, float]) -> torch.Tensor:
     """[N, S] fp32: the factor of every degree scaler for every row (scalers.py:8-29), bit-identical to what the
-    aggregation epilogue multiplies by.  Input of ``pna_linear_scaled_fwd``; cached on the CSR (a graph constant)."""
+    aggregation epilogue multiplies by.  Input of ``pna_linear_scaled_fwd``; cached on the CSR (a graph constant), except on
+    a padded CSR, whose rows change with every ``StaticBatch.build()``: computed on every call there."""
     n_scal, codes = _lib.pack_codes(scalers, _lib.SCALER_CODES, "scaler")
     key = (codes, n_scal, float(avg_deg["log"]), float(avg_deg.get("lin", 1.0)))
-    cache = csr.__dict__.setdefault("_row_scale_cache", {})
+    cache = {} if _padded(csr) else csr.__dict__.setdefault("_row_scale_cache", {})
     hit = cache.get(key)
     if hit is not None:
         capture.pin(csr, hit)
@@ -282,8 +289,12 @@ def aggregate_backward(grad_out: torch.Tensor, gathered: torch.Tensor, csr: CSRG
     grad_out = _rows2d(grad_out.to(gathered.dtype), "grad_out")
     if row_bias is not None:
         row_bias = _rows2d(row_bias.to(gathered.dtype), "row_bias")
-    deterministic = backward_mode() == "deterministic"
-    if deterministic and csr.n_edges:     # every element is written (per-slot stores, or the forward's sums per source row)
+    # a padded readout CSR has no slot-transposed CSR; every source row has at most one out-edge, so the atomic backward adds
+    # once per element and is deterministic as it is
+    deterministic = backward_mode() == "deterministic" and not (_padded(csr) and csr.sources_unique)
+    # every element is written (per-slot stores, or the forward's sums per source row), except the padding slots of a
+    # padded CSR when the messages are in CSR order: their gradient must be zero, not whatever the memory held
+    if deterministic and csr.n_edges and not (_padded(csr) and messages_in_csr_order):
         gg = torch.empty((gathered.size(0), F), dtype=torch.float32, device=dev)
     else:
         gg = torch.zeros((gathered.size(0), F), dtype=torch.float32, device=dev)
@@ -315,7 +326,7 @@ def aggregate_backward(grad_out: torch.Tensor, gathered: torch.Tensor, csr: CSRG
         return gg, gb
     # moments, the weighted sums and slot weights have no coefficient form (their per-slot gradient is not c0 + c1 * m):
     # atomic path
-    if messages_in_csr_order or csr.n_edges == 0 or csr.sources_unique or backward_mode() == "atomic" \
+    if messages_in_csr_order or csr.n_edges == 0 or csr.sources_unique or _padded(csr) or backward_mode() == "atomic" \
             or any(a in _lib.MOMENTS + _lib.WEIGHTED for a in _names(aggregators)) \
             or weights is not None \
             or 2 * _round_up(F, 4) > _lib.query(_lib.QUERY_MAX_FEATURES):

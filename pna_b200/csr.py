@@ -55,6 +55,10 @@ class CSRGraph:
     _dst: Optional[torch.Tensor] = field(default=None, repr=False)
     hot_source_fraction: float = 0.0      # pna_csr_t.hot_source_fraction: share of the gathers going to frequent sources
     sources_unique: bool = False          # every source row has at most one out-edge (readouts): the backward's atomics never collide
+    # built by pna_csr_build_padded into fixed capacities (static_batch.StaticBatch): slots past rowptr[n_nodes] are padding,
+    # no row is split, max_degree / n_light_edges are unknown on the host, and _deg / _dst are refilled in place by every
+    # StaticBatch.build()
+    padded: bool = False
 
     @property
     def device(self) -> torch.device:
@@ -71,6 +75,8 @@ class CSRGraph:
     def dst_of_slot(self) -> torch.Tensor:
         """int64 [E] destination row of each CSR slot."""
         if self._dst is None:
+            if self.padded:     # repeat_interleave leaves the tail past the real slots undefined
+                raise ValueError("a padded CSR has dst_of_slot only as StaticBatch.build() refills it")
             self._dst = torch.repeat_interleave(
                 torch.arange(self.n_nodes, device=self.device), self.in_degree.long(), output_size=self.n_edges)
         return self._dst
@@ -111,6 +117,8 @@ class CSRGraph:
         key = ("T", int(n_src))
         t = self._partials.get(key)
         if t is None:
+            if self.padded:
+                raise ValueError("a padded CSR has no transposed CSR: its backward takes the atomic or deterministic path")
             capture.guard("the transposed CSR of this graph (the coefficient backward)")
             t = build_csr(self.dst_of_slot, self.col.long(), int(n_src), n_src=self.n_nodes)
             self._partials[key] = t

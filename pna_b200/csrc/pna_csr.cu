@@ -215,6 +215,48 @@ static int light_view(const int* rowptr, const int* col, long long N, long long 
   return PNA_OK;
 }
 
+// ---- padded build (pna_csr_build_padded): fixed capacities, nothing read back -------------------------------------------------
+// status[0] error bits, [1] real edges, [2] max in-degree, [3] reserved
+__global__ void k_prepare_keys_padded(const long long* __restrict__ src, const long long* __restrict__ dst, int E, long long N,
+                                      long long NS, int* __restrict__ keys, int* __restrict__ vals, int* __restrict__ status) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= E) return;
+  const long long d = dst[e], s = src[e];
+  const bool pad = d == -1;
+  const bool bad = !pad && (d < 0 || d >= N || s < 0 || s >= NS);
+  if (bad) atomicOr(status, 1);
+  keys[e] = (pad || bad) ? (int)N : (int)d;     // padding and dropped edges sort behind every row
+  vals[e] = e;
+}
+
+// padding slots rowptr[N]..E-1 get col 0; max in-degree and the real-edge count go to the status word
+__global__ void k_padded_finish(const int* __restrict__ rowptr, long long N, int E, int* __restrict__ col, int* __restrict__ status) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int real = rowptr[N];
+  if (i < E && i >= real) col[i] = 0;
+  int deg = 0;
+  if (i < N) deg = rowptr[i + 1] - rowptr[i];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) deg = max(deg, __shfl_xor_sync(0xffffffffu, deg, o));
+  if ((threadIdx.x & 31) == 0 && deg > 0) atomicMax(status + 2, deg);
+  if (i == 0) status[1] = real;
+}
+
+// per slot: the slot-transposed build's destination key (col, or -1 = padding) and the row that owns the slot (0 = padding)
+__global__ void k_slot_rows(const int* __restrict__ rowptr, const int* __restrict__ col, long long N, int E,
+                            long long* __restrict__ transpose_dst, long long* __restrict__ dst_of_slot) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= E) return;
+  if (s >= rowptr[N]) { transpose_dst[s] = -1; dst_of_slot[s] = 0; return; }
+  long long lo = 0, hi = N;     // the last row r with rowptr[r] <= s
+  while (lo < hi) {
+    const long long mid = (lo + hi + 1) >> 1;
+    if (rowptr[mid] <= s) lo = mid; else hi = mid - 1;
+  }
+  transpose_dst[s] = col[s];
+  dst_of_slot[s] = lo;
+}
+
 // Building per-graph state reads counters back (pna_csr_build) and belongs before a CUDA graph capture, not in it: on a
 // capturing stream both builders return PNA_ERR_CAPTURING before anything is enqueued, so the capture stays intact.
 static int refuse_capture(cudaStream_t st, const char* who) {
@@ -361,5 +403,91 @@ extern "C" int pna_csr_build(const int64_t* src, const int64_t* dst, pna_csr_t* 
   csr->max_degree = host.max_degree;
   csr->n_light_edges = n_light;
   csr->hot_source_fraction = n_sample ? (float)host.hot / (float)n_sample : 0.0f;
+  return PNA_OK;
+}
+
+extern "C" int pna_csr_padded_workspace_bytes(int64_t n_nodes, int64_t n_edges, size_t* bytes) {
+  PNA_REQUIRE(bytes != nullptr, PNA_ERR_BAD_ARG, "pna_csr_padded_workspace_bytes: null out pointer");
+  PNA_REQUIRE(n_nodes >= 0 && n_edges >= 0, PNA_ERR_BAD_ARG, "pna_csr_padded_workspace_bytes: negative size");
+  PNA_REQUIRE(n_nodes < 0x7ffffffell && n_edges < 0x7fffffffll, PNA_ERR_UNSUPPORTED,
+              "pna_csr_padded_workspace_bytes: n_nodes + 1 and n_edges must be < 2^31");
+  WsLayout L;
+  const int rc = ws_layout(n_nodes + 1, n_edges, &L);     // keys 0..N: the padding sorts under the sentinel N
+  if (rc != PNA_OK) return rc;
+  *bytes = L.total;
+  return PNA_OK;
+}
+
+extern "C" int pna_csr_build_padded(const int64_t* src, const int64_t* dst, pna_csr_t* csr, int32_t* status, void* workspace,
+                                    size_t workspace_bytes, pna_stream_t stream) {
+  PNA_REQUIRE(csr != nullptr && status != nullptr, PNA_ERR_BAD_ARG, "pna_csr_build_padded: null csr/status");
+  const long long N = csr->n_nodes, E = csr->n_edges;
+  const long long NS = csr->n_src_nodes > 0 ? csr->n_src_nodes : N;
+  PNA_REQUIRE(N >= 0 && E >= 0, PNA_ERR_BAD_ARG, "pna_csr_build_padded: negative size");
+  PNA_REQUIRE(N < 0x7ffffffell && E < 0x7fffffffll && NS < 0x7fffffffll, PNA_ERR_UNSUPPORTED,
+              "pna_csr_build_padded: n_nodes + 1, n_src_nodes and n_edges must be < 2^31");
+  PNA_REQUIRE(csr->split_threshold >= 2 && (long long)csr->split_threshold > E, PNA_ERR_BAD_ARG,
+              "pna_csr_build_padded: split_threshold %d must exceed n_edges %lld (a padded CSR has no split rows)",
+              (int)csr->split_threshold, E);
+  PNA_REQUIRE(csr->rowptr != nullptr, PNA_ERR_BAD_ARG, "pna_csr_build_padded: null rowptr");
+  PNA_REQUIRE(E == 0 || (src && dst && csr->col && csr->perm), PNA_ERR_BAD_ARG, "pna_csr_build_padded: null src/dst/col/perm");
+  PNA_REQUIRE(csr->light_rowptr == nullptr || (csr->light_deg && csr->part && (E == 0 || csr->light_col) && csr->n_part >= 1),
+              PNA_ERR_BAD_ARG, "pna_csr_build_padded: light view needs light_rowptr, light_deg, light_col, part and n_part >= 1");
+  WsLayout L;
+  int rc = ws_layout(N + 1, E, &L);
+  if (rc != PNA_OK) return rc;
+  PNA_REQUIRE(workspace != nullptr && workspace_bytes >= L.total, PNA_ERR_WORKSPACE,
+              "pna_csr_build_padded: workspace %zu bytes < required %zu", workspace_bytes, L.total);
+  PNA_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255u) == 0, PNA_ERR_BAD_ARG,
+              "pna_csr_build_padded: workspace must be 256-byte aligned");
+
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  char* ws = static_cast<char*>(workspace);
+  int* keys_in = reinterpret_cast<int*>(ws + L.keys_in);
+  int* keys_out = reinterpret_cast<int*>(ws + L.keys_out);
+  int* vals_in = reinterpret_cast<int*>(ws + L.vals_in);
+  PNA_CUDA_TRY(cudaMemsetAsync(status, 0, 4 * sizeof(int32_t), st));
+  const int TB = 256;
+  if (E > 0) {
+    const int nE = (int)E;
+    const unsigned gE = (unsigned)((E + TB - 1) / TB);
+    k_prepare_keys_padded<<<gE, TB, 0, st>>>(reinterpret_cast<const long long*>(src), reinterpret_cast<const long long*>(dst), nE,
+                                             N, NS, keys_in, vals_in, status);
+    PNA_CUDA_TRY(cudaGetLastError());
+    size_t cub_bytes = L.cub_bytes;
+    PNA_CUDA_TRY(cub::DeviceRadixSort::SortPairs(ws + L.cub_temp, cub_bytes, (const int*)keys_in, keys_out, (const int*)vals_in,
+                                                  csr->perm, nE, 0, key_bits(N + 1), st));
+    k_fill_col<<<gE, TB, 0, st>>>(reinterpret_cast<const long long*>(src), csr->perm, nE, NS, csr->col);
+    PNA_CUDA_TRY(cudaGetLastError());
+  }
+  k_rowptr<<<(unsigned)((N + 1 + TB - 1) / TB), TB, 0, st>>>(keys_out, (int)E, N, csr->rowptr);
+  PNA_CUDA_TRY(cudaGetLastError());
+  const long long n_fin = N > E ? N : E;
+  k_padded_finish<<<(unsigned)((n_fin + TB) / TB), TB, 0, st>>>(csr->rowptr, N, (int)E, csr->col, status);
+  PNA_CUDA_TRY(cudaGetLastError());
+  if (csr->light_rowptr) {
+    ChunkRows none = {nullptr, nullptr, nullptr, 1};
+    rc = light_view(csr->rowptr, csr->col, N, N, csr->split_threshold, nullptr, none, csr->n_part, csr->light_rowptr,
+                    csr->light_deg, csr->light_col, csr->part, keys_in, ws + L.cub_temp, L.cub_bytes, st);
+    if (rc != PNA_OK) return rc;
+  }
+  csr->n_hubs = 0;
+  csr->n_chunks = 0;
+  csr->max_degree = 0;        // on the device: status[2]
+  csr->n_light_edges = 0;     // on the device: status[1] (= light_rowptr[n_nodes])
+  csr->hot_source_fraction = 0.0f;
+  return PNA_OK;
+}
+
+extern "C" int pna_csr_slot_rows(const int32_t* rowptr, const int32_t* col, int64_t n_rows, int64_t n_slots, int64_t* transpose_dst,
+                                 int64_t* dst_of_slot, pna_stream_t stream) {
+  PNA_REQUIRE(n_rows >= 0 && n_slots >= 0 && n_rows < 0x7fffffffll && n_slots < 0x7fffffffll, PNA_ERR_BAD_ARG,
+              "pna_csr_slot_rows: bad sizes");
+  if (n_slots == 0) return PNA_OK;
+  PNA_REQUIRE(rowptr && col && transpose_dst && dst_of_slot, PNA_ERR_BAD_ARG, "pna_csr_slot_rows: null pointer");
+  const int TB = 256;
+  k_slot_rows<<<(unsigned)((n_slots + TB - 1) / TB), TB, 0, static_cast<cudaStream_t>(stream)>>>(
+      rowptr, col, n_rows, (int)n_slots, reinterpret_cast<long long*>(transpose_dst), reinterpret_cast<long long*>(dst_of_slot));
+  PNA_CUDA_TRY(cudaGetLastError());
   return PNA_OK;
 }

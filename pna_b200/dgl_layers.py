@@ -31,6 +31,7 @@ from .aggregate import pna_aggregate, row_scales
 from .edge_mlp import edge_messages
 from .linear import compact_path_ok, post_linear_towers_scaled
 from .graph import graph_csr
+from .static_batch import StaticBatch
 from .nn_blocks import FCLayer, MLP
 from .towers import TowerLayer
 
@@ -64,7 +65,7 @@ class PNATower(nn.Module):
         self.posttrans = MLP(in_size=(len(aggregators) * len(scalers) + 1) * in_dim, hidden_size=out_dim, out_size=out_dim,
                              layers=posttrans_layers, mid_activation="relu", last_activation="none")
 
-    def finish(self, h_cat, snorm_n, blocks=None, fp=None):
+    def finish(self, h_cat, snorm_n, blocks=None, fp=None, g=None):
         """posttrans -> graph norm -> batch norm -> dropout (pna_layer.py:67-76).  h_cat may carry padded column blocks
         (width fp instead of in_dim): the first posttrans Linear then gets zero weight columns at the pad positions."""
         if fp is not None and fp != self.in_dim:
@@ -72,21 +73,21 @@ class PNATower(nn.Module):
             h = self.posttrans(h_cat, first_weight=w0)
         else:
             h = self.posttrans(h_cat)
-        return self._norms(h, snorm_n)
+        return self._norms(h, snorm_n, g)
 
-    def finish_linear(self, h, snorm_n):
+    def finish_linear(self, h, snorm_n, g=None):
         """``finish`` from the output of the first posttrans Linear (computed for every tower at once by PNALayer)."""
         fcs = self.posttrans.fully_connected
         h = fcs[0].after_linear(h)
         for fc in list(fcs)[1:]:
             h = fc(h)
-        return self._norms(h, snorm_n)
+        return self._norms(h, snorm_n, g)
 
-    def _norms(self, h, snorm_n):
+    def _norms(self, h, snorm_n, g=None):
         if self.graph_norm:
             h = h * snorm_n
-        if self.batch_norm:
-            h = self.batchnorm_h(h)
+        if self.batch_norm:     # a StaticBatch: statistics over its real rows only
+            h = g.batch_norm(self.batchnorm_h, h) if isinstance(g, StaticBatch) else self.batchnorm_h(h)
         return F.dropout(h, self.dropout, training=self.training)
 
 
@@ -167,11 +168,11 @@ class PNALayer(TowerLayer, nn.Module):
             # the rest of each tower's posttrans and norms on its output_tower slice of the towers' first posttrans Linear
             y = post_linear_towers_scaled(agg, row_scales(csr, self.scalers, self.avg_d), *self._post_weights(fp))
             ot = self.output_tower
-            h_cat = torch.cat([tw.finish_linear(y[:, t * ot:(t + 1) * ot], snorm_n) for t, tw in enumerate(self.towers)], dim=1)
+            h_cat = torch.cat([tw.finish_linear(y[:, t * ot:(t + 1) * ot], snorm_n, g) for t, tw in enumerate(self.towers)], dim=1)
         else:
             blocks = 1 + len(self.aggregators) * len(self.scalers)
             agg = agg.view(h.size(0), len(self.towers), -1)                # [N, T, (1 + S*A) * fp] = cat([h_t, reduced])
-            h_cat = torch.cat([tw.finish(agg[:, t], snorm_n, blocks, fp) for t, tw in enumerate(self.towers)], dim=1)
+            h_cat = torch.cat([tw.finish(agg[:, t], snorm_n, blocks, fp, g) for t, tw in enumerate(self.towers)], dim=1)
         h_out = self.mixing_network(h_cat)
         if self.residual:
             h_out = h_in + h_out
@@ -215,7 +216,7 @@ class PNASimpleLayer(nn.Module):
             agg = pna_aggregate(hp, csr, self.aggregators, self.scalers, self.avg_d, zero_isolated=True, relu_var=True)
             h = self.posttrans(agg, first_weight=w0)
         if self.batch_norm:
-            h = self.batchnorm_h(h)
+            h = g.batch_norm(self.batchnorm_h, h) if isinstance(g, StaticBatch) else self.batchnorm_h(h)
         h = F.relu(h)
         if self.residual:
             h = h_in + h

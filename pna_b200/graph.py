@@ -13,6 +13,7 @@ import torch
 
 from . import capture
 from .csr import CSRGraph, build_csr, tensor_version
+from .static_batch import StaticBatch
 
 _ATTR = "_pna_b200_csr"
 
@@ -60,7 +61,13 @@ def graph_num_nodes(g) -> int:
 
 
 def graph_csr(g, device: torch.device) -> CSRGraph:
-    """CSR of the graph on `device`, built on first use and cached on the object."""
+    """CSR of the graph on `device`, built on first use and cached on the object.  A ``StaticBatch`` hands out its padded
+    CSR (built by its ``build()``), with no cache lookup."""
+    if isinstance(g, StaticBatch):
+        if g.device != device:
+            raise ValueError(f"the StaticBatch lives on {g.device}, the features on {device}")
+        capture.pin(g)
+        return g.csr
     src, dst = graph_edges(g)
     n = graph_num_nodes(g)
     # a graph mutated in place (add_edges / remove_edges / add_self_loop) hands out different edge tensors or counts:

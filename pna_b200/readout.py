@@ -18,13 +18,21 @@ import torch
 from . import capture
 from .aggregate import at_boundary, pna_aggregate
 from .csr import CSRGraph, build_csr, tensor_version
+from .static_batch import StaticBatch, of_batch
 
 _UNIT = {"log": 1.0, "lin": 1.0}        # identity scaler only: the averages are never read
 _CACHE: "OrderedDict[tuple, tuple]" = OrderedDict()
 
 
 def batch_csr(batch: torch.Tensor, n_graphs: int) -> CSRGraph:
-    """CSR whose row g lists the nodes of graph g; cached on the identity of ``batch`` (one per mini-batch)."""
+    """CSR whose row g lists the nodes of graph g; cached on the identity of ``batch`` (one per mini-batch).  The ``batch``
+    tensor of a ``StaticBatch`` is recognised by identity (``copy_`` bumps its version) and gets its padded readout CSR."""
+    sb = of_batch(batch)
+    if sb is not None:
+        if int(n_graphs) != sb.max_graphs:
+            raise ValueError(f"a StaticBatch's batch tensor reduces into its max_graphs = {sb.max_graphs} rows, not {n_graphs}")
+        capture.pin(sb)
+        return sb.readout_csr
     key = (batch.data_ptr(), tensor_version(batch), int(batch.numel()), int(n_graphs), str(batch.device))
     hit = _CACHE.get(key)
     if hit is not None:
@@ -46,6 +54,8 @@ def segment_reduce(x: torch.Tensor, batch: torch.Tensor, n_graphs: Optional[int]
         raise KeyError(reduce)
     if x.dim() != 2 or batch.dim() != 1 or batch.numel() != x.size(0):
         raise ValueError("x must be [N, F] and batch [N]")
+    if n_graphs is None and of_batch(batch) is not None:
+        n_graphs = of_batch(batch).max_graphs
     if n_graphs is None:
         capture.guard("a readout without its graph count (int(batch.max()) reads back)", "pass n_graphs / size")
         n_graphs = int(batch.max()) + 1 if batch.numel() else 0
@@ -65,6 +75,8 @@ def global_max_pool(x: torch.Tensor, batch: torch.Tensor, size: Optional[int] = 
 
 
 def _graph_batch(g, device) -> tuple:
+    if isinstance(g, StaticBatch):       # padded nodes are in no graph, graph rows past the real count come out zero
+        return g.batch, g.max_graphs
     sizes = getattr(g, "batch_num_nodes", None)
     sizes = sizes() if callable(sizes) else sizes
     sizes = torch.as_tensor(sizes, dtype=torch.long)

@@ -192,3 +192,23 @@ def powerlaw_stream(n_nodes: int, n_edges: int, device, seed: int = 0, alpha: fl
     for e0 in range(0, n_edges, chunk):
         c = min(chunk, n_edges - e0)
         yield perm_s[zipf_ids(c)], perm_d[zipf_ids(c)]
+
+
+def sub_batch(edge_index: torch.Tensor, node_graph: torch.Tensor, graph_ids: torch.Tensor):
+    """The mini-batch of graphs ``graph_ids`` (in that order) of a batched graph, as a shuffling data loader collates it:
+    (edge_index renumbered from 0, batch_num_nodes, the node ids and the edge ids it took).  Edges are kept in their
+    order within each graph."""
+    n_graphs = int(node_graph.max()) + 1
+    sizes = torch.bincount(node_graph, minlength=n_graphs)
+    offs = torch.cumsum(sizes, 0) - sizes
+    graph_ids = graph_ids.long()
+    sub = sizes[graph_ids]
+    node_ids = torch.repeat_interleave(offs[graph_ids] - (torch.cumsum(sub, 0) - sub), sub) + torch.arange(int(sub.sum()))
+    new_id = torch.full((node_graph.numel(),), -1, dtype=torch.long)
+    new_id[node_ids] = torch.arange(node_ids.numel())
+    rank = torch.full((n_graphs,), -1, dtype=torch.long)
+    rank[graph_ids] = torch.arange(graph_ids.numel())
+    er = rank[node_graph[edge_index[1]]]
+    eids = (er >= 0).nonzero().flatten()
+    eids = eids[torch.sort(er[eids], stable=True).indices]
+    return new_id[edge_index[:, eids]], sub, node_ids, eids
