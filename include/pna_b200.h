@@ -542,6 +542,32 @@ int pna_linear_towers_scaled_fwd_bf16(const void* a, int64_t lda, const float* r
                                       const float* bias, float* y, int64_t ldy, int64_t n_rows, int32_t n_towers, int32_t n_feat,
                                       int32_t n_aggr, int32_t n_out, pna_stream_t stream);
 
+/* ---- Set2Set graph readout (reference models/layers.py:53-98, the readout of S2SReadout) --------------------------------
+ * x [n_graphs, n_nodes, n_feat = D] fp32 contiguous; the LSTM is nn.LSTM(2D, D, num_layers=1) with PyTorch's gate order
+ * i, f, g, o: w_ih [4D, 2D], w_hh [4D, D], b_ih [4D], b_hh [4D], all contiguous.  With h, c, q* = 0 at the start, each of
+ * the `steps` steps computes
+ *     q, (h, c) = LSTM(q*, (h, c));   e_i = x_i . q;   alpha = softmax_i(e) (maximum subtracted);   r = sum_i alpha_i x_i;
+ *     q* = [q, r]
+ * and out [n_graphs, 2D] is q* after the last step.  One CTA per graph runs every step; no atomics, every sum in an order
+ * fixed by the shape, so the results are a fixed function of the inputs.
+ * saved (the forward writes it when non-NULL; the backward reads it): pna_set2set_saved_floats floats, one record of
+ * 7D + n_nodes floats per step t and graph b, record index t * n_graphs + b:
+ *     [ q*_t (2D) | c_t (D) | i_t f_t g_t o_t, the gate activations (4D) | alpha_t (n_nodes) ]
+ * so the records' first 2D floats, at a pitch of 7D + n_nodes, are the matrix Q* [steps * n_graphs, 2D].
+ * pna_set2set_bwd, from grad_out [n_graphs, 2D], writes grad_x [n_graphs, n_nodes, D] (NULL: not computed) and the
+ * pre-activation gate gradients grad_gates [steps, n_graphs, 4D] (gate order i, f, g, o).  The weight gradients are then
+ * GEMMs over the steps * n_graphs rows: dW_ih = dG[1:]^T Q*[:-1], dW_hh = dG[1:]^T Q*[:-1, :D] (steps shifted by one; the
+ * input of step 0 is zero) and db_ih = db_hh = sum of dG over all rows.
+ * Limits: 1 <= n_feat <= 128, n_nodes * n_feat <= 16384, n_graphs < 2^31, else PNA_ERR_UNSUPPORTED; a size <= 0 or a
+ * null pointer: PNA_ERR_BAD_ARG.  No alignment is required.  The calls allocate nothing, read nothing back and do not
+ * synchronise, so they may be enqueued on a stream that is capturing a CUDA graph.  (Appended in ABI version 8.) */
+int pna_set2set_saved_floats(int64_t n_graphs, int32_t n_nodes, int32_t n_feat, int32_t steps, int64_t* n_floats);
+int pna_set2set_fwd(const float* x, int64_t n_graphs, int32_t n_nodes, int32_t n_feat, int32_t steps, const float* w_ih,
+                    const float* w_hh, const float* b_ih, const float* b_hh, float* out, float* saved, pna_stream_t stream);
+int pna_set2set_bwd(const float* x, int64_t n_graphs, int32_t n_nodes, int32_t n_feat, int32_t steps, const float* w_ih,
+                    const float* w_hh, const float* saved, const float* grad_out, float* grad_x, float* grad_gates,
+                    pna_stream_t stream);
+
 int pna_query(int what);
 const char* pna_last_error(void);
 

@@ -12,9 +12,10 @@ from .pyg import PNAConv, PNAConvSimple
 from .graph import Graph, avg_d_from_graphs, graph_csr
 from .dgl_layers import PNALayer, PNASimpleLayer
 from .static_batch import StaticBatch
+from .set2set import S2SReadout, Set2Set
 from . import capture, dense, padding, readout
 
 __all__ = ["PnaError", "CaptureError", "build_library", "aggregate_forward", "avg_deg_from_histogram", "pna_aggregate", "CSRGraph",
            "build_csr", "clear_csr_cache", "csr_from_edge_index", "PNAConv", "PNAConvSimple", "Graph", "avg_d_from_graphs",
-           "graph_csr", "PNALayer", "PNASimpleLayer", "StaticBatch", "capture", "dense", "readout"]
+           "graph_csr", "PNALayer", "PNASimpleLayer", "StaticBatch", "Set2Set", "S2SReadout", "capture", "dense", "readout"]
 __version__ = "0.1.0"

@@ -17,7 +17,7 @@ LIB_PATH = os.environ.get("PNA_B200_LIB") or os.path.join(_HERE, "libpna_sm90.so
 CUDA_SOURCES = [os.path.join(_HERE, "csrc", n) for n in
                 ("pna_aggregate.cu", "pna_aggregate_f32_vec.cu", "pna_aggregate_f32_scalar.cu", "pna_aggregate_bf16_vec.cu",
                  "pna_aggregate_bf16_scalar.cu", "pna_aggregate_bwd.cu", "pna_linear.cu", "pna_csr.cu", "pna_peer.cu", "pna_misc.cu",
-                 "pna_edge_mlp.cu")]
+                 "pna_edge_mlp.cu", "pna_set2set.cu")]
 CUDA_HEADERS = [os.path.join(_HERE, "csrc", n) for n in ("common.cuh", "pna_aggregate.cuh", "pna_aggregate_impl.cuh",
                                                                    "pna_aggregate_moments.cuh", "pna_aggregate_weighted.cuh",
                                                                    "pna_aggregate_adj_weight.cuh")] + [
@@ -47,6 +47,7 @@ FLAG_ZERO_ISOLATED, FLAG_SKIP_LIGHT, FLAG_SKIP_HUBS, FLAG_RELU_VAR, FLAG_GATHER_
 (QUERY_ABI_VERSION, QUERY_SM_ARCH, QUERY_DEFAULT_SPLIT, QUERY_DEFAULT_CHUNK, QUERY_DEVICE_SM_COUNT,
  QUERY_MAX_FEATURES, QUERY_SIZEOF_CSR, QUERY_SIZEOF_AGG) = range(8)
 EDGE_MLP_MAX_WIDTH = 64      # PNA_EDGE_MLP_MAX_WIDTH
+SET2SET_MAX_FEAT, SET2SET_MAX_ELEMS = 128, 16384     # pna_set2set_*: n_feat <= 128, n_nodes * n_feat <= 16384
 
 # every symbol the header declares (checked by tests/test_abi.py)
 EXPORTED_SYMBOLS = ("pna_csr_workspace_bytes", "pna_csr_build", "pna_csr_light_view", "pna_csr_light_view_workspace_bytes", "pna_aggregate_fwd", "pna_aggregate_bwd",
@@ -56,7 +57,8 @@ EXPORTED_SYMBOLS = ("pna_csr_workspace_bytes", "pna_csr_build", "pna_csr_light_v
                     "pna_edge_mlp_bwd", "pna_edge_msg_fwd", "pna_edge_msg_bwd", "pna_query", "pna_last_error",
                     "pna_linear_towers_scaled_fwd", "pna_linear_towers_bwd_data", "pna_edge_msg_fwd_bf16", "pna_edge_msg_bwd_bf16",
                     "pna_linear_towers_scaled_fwd_bf16", "pna_aggregate_fwd_weighted", "pna_aggregate_bwd_weighted",
-                    "pna_aggregate_bwd_slots_weighted", "pna_csr_padded_workspace_bytes", "pna_csr_build_padded", "pna_csr_slot_rows")
+                    "pna_aggregate_bwd_slots_weighted", "pna_csr_padded_workspace_bytes", "pna_csr_build_padded", "pna_csr_slot_rows",
+                    "pna_set2set_saved_floats", "pna_set2set_fwd", "pna_set2set_bwd")
 
 
 class PnaError(RuntimeError):
@@ -255,6 +257,14 @@ def lib() -> C.CDLL:
         L.pna_edge_msg_bwd_bf16.argtypes = L.pna_edge_msg_bwd.argtypes
         L.pna_linear_towers_scaled_fwd_bf16.restype = C.c_int
         L.pna_linear_towers_scaled_fwd_bf16.argtypes = L.pna_linear_towers_scaled_fwd.argtypes
+        L.pna_set2set_saved_floats.restype = C.c_int
+        L.pna_set2set_saved_floats.argtypes = [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int64)]
+        L.pna_set2set_fwd.restype = C.c_int
+        L.pna_set2set_fwd.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.pna_set2set_bwd.restype = C.c_int
+        L.pna_set2set_bwd.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         abi = L.pna_query(QUERY_ABI_VERSION)
         if abi != ABI_VERSION:
             raise ImportError(f"{LIB_PATH} has ABI version {abi}, this package needs {ABI_VERSION}: rebuild it")
